@@ -152,6 +152,19 @@ int mg_host_threads(const mg_env *env);
  * (10, 0, agent_dir). out_dev: uint8[n][W][H][3]. */
 int mg_full_obs(mg_env *env, uint8_t *out_dev, void *stream);
 
+/* Replaces: MiniGridEnv.hash (minigrid_env.py:159-170) for every env, before its truncation to `size` hex digits:
+ * digest_dev uint8[n][32] = SHA-256(str(grid.encode().tolist()) + str(agent_pos) + str(agent_dir)). Reads the grid and
+ * the agent records only; ordered on `stream` like every other entry point.
+ * str(agent_pos) depends on how the reference last assigned agent_pos, and the engine reproduces that rule:
+ *  - after a forward move that succeeded since the last reset (minigrid_env.py:553, tuple(agent_pos + dir_vec)), and
+ *    after mg_set_state with agent records: a tuple of numpy ints, "(np.int64(3), np.int64(12))";
+ *  - otherwise the form the kind's generator leaves: a tuple of ints "(1, 1)" for the fixed starts (empty.py:109,
+ *    distshift.py:115, dynamicobstacles.py:123), numpy's str(ndarray) "[ 3 10]" for crossing.py:141, lavagap.py:110
+ *    and memory.py:129, and a tuple of numpy ints for every generator that calls place_agent / place_obj
+ *    (minigrid_env.py:347-350, 383-395).
+ * The "moved" state is not part of mg_get_state's output. */
+int mg_hash(mg_env *env, uint8_t *digest_dev, void *stream);
+
 /* The reference's observation wrappers (minigrid/wrappers.py) for the whole batch, on the device. `image_dev` is the
  * observation image the last mg_step / mg_reset / mg_gen_obs wrote (uint8[n][V][V][3]).
  *  mg_obs_view         ViewSizeWrapper.observation (:663-673): gen_obs with agent_view_size = view_size (odd, 3..15);

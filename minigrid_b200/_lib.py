@@ -16,7 +16,7 @@ EXPORTS = [
     "mg_create", "mg_destroy", "mg_last_error", "mg_num_envs", "mg_launch_count", "mg_seed", "mg_seed_base",
     "mg_reset", "mg_seed_masked", "mg_reset_masked", "mg_step", "mg_gen_obs", "mg_reset_host", "mg_step_host", "mg_full_obs", "mg_get_state", "mg_set_state",
     "mg_check_error", "mg_profile", "mg_profile_read", "mg_set_host_format", "mg_host_d2h_bytes", "mg_host_threads", "mg_expand_packed", "mg_expand_packed_mt", "mg_obs_view", "mg_obs_onehot", "mg_obs_flat", "mg_obs_symbolic",
-    "mg_obs_rgb_partial", "mg_obs_rgb_full",
+    "mg_obs_rgb_partial", "mg_obs_rgb_full", "mg_hash",
 ]
 
 
@@ -60,6 +60,7 @@ def load(build_if_missing: bool = True):
     L.mg_reset_host.argtypes = [p, p, p]
     L.mg_step_host.argtypes = [p] * 7
     L.mg_full_obs.argtypes = [p, p, p]
+    L.mg_hash.argtypes = [p, p, p]
     L.mg_set_host_format.argtypes = [p, i32, i32]
     L.mg_host_d2h_bytes.restype = i64
     L.mg_host_d2h_bytes.argtypes = [p]

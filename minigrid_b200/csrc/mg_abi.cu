@@ -11,6 +11,7 @@
 
 #include "../../include/minigrid_b200.h"
 #include "mg_common.cuh"
+#include "mg_hash.cuh"
 #include "mg_obs.cuh"
 #include "mg_host_expand.h"
 
@@ -36,6 +37,8 @@ cudaError_t launch_symbolic(const Params &p, long long *out, cudaStream_t s);
 cudaError_t launch_rgb_partial(const uint8_t *img, const uint8_t *tiles, const uint16_t *index, uint8_t *out, long long n_envs, cudaStream_t s);
 cudaError_t launch_rgb_full(const Params &p, const uint8_t *img, const uint8_t *tiles, const uint16_t *index, uint8_t *out, cudaStream_t s);
 cudaError_t launch_template(const Params &p, uint32_t *tmpl, cudaStream_t stream);
+cudaError_t configure_hash(const Params &p, int *grid);
+cudaError_t launch_hash(const Params &p, int grid, const uint4 *tmpl, int form0, uint8_t *digest, cudaStream_t stream);
 }  // namespace mg
 
 using namespace mg;
@@ -76,6 +79,9 @@ struct mg_env {
   // optional per-launch timing of K1 (bench.py's roofline leg)
   int profiling;
   std::vector<cudaEvent_t> *prof_events;  // start/stop pairs
+  // MiniGridEnv.hash (mg_hash.cu): the prefix template of this geometry, the kind's form of agent_pos after a reset
+  const uint4 *d_hash_tmpl;
+  int hash_form, hash_grid;
 };
 
 static thread_local std::string g_err;
@@ -226,7 +232,9 @@ int mg_create(int kind, int width, int height, int max_steps, int see_through_wa
   const size_t sz_tmpl = align_up((size_t)p.g.wpe * 4, 256);
   const size_t sz_hot = align_up((size_t)p.n_tiles, 256);
   const size_t sz_extra = kind == MG_KIND_DYNOBS ? align_up(n_pad * sizeof(uint4), 256) : 0;
-  const size_t total = sz_grid + sz_agent + sz_rng + 256 /*err*/ + sz_lut_r + 1024 + VIS_TBL_BYTES + sz_tmpl + sz_hot + sz_extra;
+  const size_t n_hash = (size_t)hash_shape(width, height).nwords;
+  const size_t sz_hash = align_up(n_hash * sizeof(uint4), 256);
+  const size_t total = sz_grid + sz_agent + sz_rng + 256 /*err*/ + sz_lut_r + 1024 + VIS_TBL_BYTES + sz_tmpl + sz_hot + sz_extra + sz_hash;
   cudaError_t e = cudaMalloc(&h->d_arena, total);
   if (e != cudaSuccess) { delete h; return fail(MG_ERR_CUDA, std::string("cudaMalloc arena: ") + cudaGetErrorString(e)); }
   uint8_t *base = (uint8_t *)h->d_arena;
@@ -239,7 +247,10 @@ int mg_create(int kind, int width, int height, int max_steps, int see_through_wa
   uint16_t *d_vt = (uint16_t *)base; base += VIS_TBL_BYTES;
   uint32_t *d_tm = (uint32_t *)base; base += sz_tmpl;
   p.tile_hot = base; base += sz_hot;
-  p.extra = sz_extra ? (uint4 *)base : nullptr;
+  p.extra = sz_extra ? (uint4 *)base : nullptr; base += sz_extra;
+  uint4 *d_ht = (uint4 *)base;
+  h->d_hash_tmpl = d_ht;
+  h->hash_form = hash_initial_form(kind, p.kp);
   p.reward_lut = d_rl; p.cell_lut = d_cl; p.vis_tbl = d_vt; p.tmpl = d_tm;
 
   // _reward(): 1 - 0.9 * (step_count / max_steps) in host IEEE double, never contracted (minigrid_env.py:245)
@@ -262,10 +273,14 @@ int mg_create(int kind, int width, int height, int max_steps, int see_through_wa
     build_vis_table(vt);
     if (e == cudaSuccess) e = cudaMemcpy(d_vt, vt, VIS_TBL_BYTES, cudaMemcpyHostToDevice);
     free(vt);
+    std::vector<uint4> ht(n_hash);
+    build_hash_template(width, height, p.g.lswC, ht.data());
+    if (e == cudaSuccess) e = cudaMemcpy(d_ht, ht.data(), n_hash * sizeof(uint4), cudaMemcpyHostToDevice);
   }
   if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&h->hstream, cudaStreamNonBlocking);
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&h->ev_order, cudaEventDisableTiming);
   if (e == cudaSuccess) e = configure_step(p, &h->plan);
+  if (e == cudaSuccess) e = configure_hash(p, &h->hash_grid);
   if (e == cudaSuccess && getenv("MINIGRID_B200_VERBOSE"))
     fprintf(stderr, "[minigrid_b200] K1 plan: layout=%d, %d warps/CTA, vis=%d, nbuf=%d, %d CTA/SM, grid=%d, smem=%zu B, tiles=%d\n", p.g.layout, h->plan.warps,
             h->plan.vis, h->plan.nbuf, h->plan.ctas_per_sm, h->plan.grid, h->plan.smem, p.n_tiles);
@@ -475,6 +490,15 @@ int mg_full_obs(mg_env *h, uint8_t *out_dev, void *stream) {
   MG_ON_DEVICE(h);
   note_stream(h, (cudaStream_t)stream);
   MG_CUDA(launch_full_obs(h->p, out_dev, 1, (cudaStream_t)stream));
+  h->launches += 1;
+  return MG_OK;
+}
+
+int mg_hash(mg_env *h, uint8_t *digest_dev, void *stream) {
+  if (!h || !digest_dev) return fail(MG_ERR_INVALID_ARG, "mg_hash: NULL argument");
+  MG_ON_DEVICE(h);
+  note_stream(h, (cudaStream_t)stream);
+  MG_CUDA(launch_hash(h->p, h->hash_grid, h->d_hash_tmpl, h->hash_form, digest_dev, (cudaStream_t)stream));
   h->launches += 1;
   return MG_OK;
 }

@@ -60,6 +60,9 @@ constexpr uint32_t CODE_LAVA = T_LAVA | (C_RED << 4);
 
 // agent flags (second word of the agent record, bits 8..)
 constexpr uint32_t FLAG_PENDING = 2u;  // episode ended last step (SyncVectorEnv._autoreset_envs[i], NEXT_STEP)
+// a forward move succeeded since the last reset, or the agent record was injected (mg_set_state): agent_pos is then a
+// tuple of numpy ints (minigrid_env.py:553), which MiniGridEnv.hash() prints differently (mg_hash.cuh)
+constexpr uint32_t FLAG_MOVED = 1u;
 
 enum : int { KIND_EMPTY = 0, KIND_DOORKEY = 1, KIND_CROSSING = 2, KIND_FOURROOMS = 3, KIND_LAVAGAP = 4, KIND_DISTSHIFT = 5,
              KIND_MULTIROOM = 6,

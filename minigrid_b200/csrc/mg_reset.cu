@@ -38,7 +38,7 @@ k_reset(Params p, const uint8_t *__restrict__ mask, uint8_t *__restrict__ obs, i
     fill_level<KIND>(p, L, env);
     uint4 rec;
     rec.x = (uint32_t)L.ax | ((uint32_t)L.ay << 8);
-    rec.y = (uint32_t)L.adir;  // flags cleared: SyncVectorEnv.reset() clears _autoreset_envs
+    rec.y = (uint32_t)L.adir;  // flags cleared: SyncVectorEnv.reset() clears _autoreset_envs; FLAG_MOVED: the generator placed the agent
     if (has_post_filter<KIND>()) {  // post-filter targets in the spare bits (mg_postfilter.cuh)
       rec.x |= ((uint32_t)level_tx(L) << 16) | ((uint32_t)level_ty(L) << 24);
       rec.y |= level_aux(L) << 16;

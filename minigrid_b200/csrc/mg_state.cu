@@ -156,7 +156,7 @@ __global__ void k_set_agent(Params p, const int32_t *__restrict__ agent, const u
       return;  // record, rng and pending flag of this env stay as they were
     }
     rec.x = (rec.x & 0xFFFF0000u) | (uint32_t)(a[0] & 0xFF) | ((uint32_t)(a[1] & 0xFF) << 8);  // keeps the post-filter targets
-    rec.y = (rec.y & ~3u) | (uint32_t)(a[2] & 3);
+    rec.y = (rec.y & ~3u) | (uint32_t)(a[2] & 3) | (FLAG_MOVED << 8);  // an injected position hashes as a tuple of numpy ints
     rec.z = a[3] >= 0 ? ((uint32_t)(a[3] & 15) | ((uint32_t)(a[4] & 7) << 4)) : 0u;
     rec.w = (uint32_t)a[5];
   }

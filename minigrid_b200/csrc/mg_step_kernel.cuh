@@ -469,7 +469,7 @@ k_step(const __grid_constant__ Params p, const void *__restrict__ actions, int a
 #endif
         const ResetOut ro = warp_reset<KIND>(p, pend, tile, WIN ? nullptr : gtile, lane);
         if (fresh) {
-          ax = ro.ax; ay = ro.ay; dir = ro.dir; carry = 0; steps = 0; flags &= ~FLAG_PENDING;
+          ax = ro.ax; ay = ro.ay; dir = ro.dir; carry = 0; steps = 0; flags &= ~(FLAG_PENDING | FLAG_MOVED);
           if (PF) { tx = ro.tx; ty = ro.ty; flags = (flags & 0xFFu) | (ro.aux << 8); }
         }
       }
@@ -530,7 +530,7 @@ k_step(const __grid_constant__ Params p, const void *__restrict__ actions, int a
 
       const uint32_t carry_before = carry;
       const int act = pre_filter<KIND>(action);
-      const StepOut so = transition(act, fc, fx, fy, ax, ay, dir, carry);
+      const StepOut so = transition(act, fc, fx, fy, ax, ay, dir, carry, &flags);
       const uint32_t newc = so.newc;
       terminated = so.terminated;
       if (so.goal)  // _reward(), minigrid_env.py:240-245: host-computed table, never an FMA
@@ -617,7 +617,7 @@ k_step(const __grid_constant__ Params p, const void *__restrict__ actions, int a
         wrote = true;
         const ResetOut ro = warp_reset<KIND>(p, pend, tile, WIN ? nullptr : gtile, lane);
         if (again) {
-          ax = ro.ax; ay = ro.ay; dir = ro.dir; carry = 0; steps = 0;
+          ax = ro.ax; ay = ro.ay; dir = ro.dir; carry = 0; steps = 0; flags &= ~FLAG_MOVED;
           if (PF) { tx = ro.tx; ty = ro.ty; flags = (flags & 0xFFu) | (ro.aux << 8); }
         }
         if (WIN && again) load_view_words(g, ax, ay, dir, vw, ldw);  // the regenerated level replaces the loaded words

@@ -20,9 +20,11 @@ MG_HD void front_pos(const Geom &g, int ax, int ay, int dir, int &fx, int &fy) {
   fy = clampi(ay + dy, 0, g.H - 1);
 }
 
+// flags: the agent flags (mg_common.cuh), if given; a forward move that succeeds sets FLAG_MOVED in them.
 // Straight-line (select-based) form: every lane runs the same instructions whatever its action, so a warp of
 // 32 environments with 32 different actions does not diverge.
-MG_HD StepOut transition(int action, uint32_t fc, int fx, int fy, int &ax, int &ay, int &dir, uint32_t &carry) {
+MG_HD StepOut transition(int action, uint32_t fc, int fx, int fy, int &ax, int &ay, int &dir, uint32_t &carry,
+                         uint32_t *flags = nullptr) {
   StepOut o;
   const uint32_t t4 = fc & 15u, col = (fc >> 4) & 7u;
   const bool isF = action == A_FORWARD, isP = action == A_PICKUP, isD = action == A_DROP, isT = action == A_TOGGLE;
@@ -32,6 +34,7 @@ MG_HD StepOut transition(int action, uint32_t fc, int fx, int fy, int &ax, int &
   const bool mv = isF && ((0x031Au >> t4) & 1u);
   ax = mv ? fx : ax;
   ay = mv ? fy : ay;
+  if (flags) *flags |= mv ? FLAG_MOVED : 0u;  // agent_pos = tuple(fwd_pos) (:553): MiniGridEnv.hash prints numpy ints from now on
   o.goal = (isF && t4 == T_GOAL) ? 1u : 0u;
   o.terminated = (isF && (t4 == T_GOAL || t4 == T_LAVA)) ? 1u : 0u;
   // pickup: can_pickup = Key, Ball, Box, and nothing carried                               :561-566

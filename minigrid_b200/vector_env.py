@@ -256,6 +256,28 @@ class MinigridVecEnv(_VectorEnvBase):
             _lib.check(self._L.mg_full_obs(self._h, self._p(out), self._stream()))
         return out
 
+    def hash_digest(self, out: torch.Tensor | None = None):
+        """MiniGridEnv.hash (minigrid_env.py:159-170) of every env as the raw SHA-256 digest: uint8[n, 32] on the device,
+        enqueued on the current stream. The first 8 bytes viewed as int64 make a state key for counting bonuses."""
+        if out is None:
+            out = torch.empty((self.num_envs, 32), dtype=torch.uint8, device=self.device)
+        elif out.shape != (self.num_envs, 32) or out.dtype != torch.uint8 or out.device != self.device or not out.is_contiguous():
+            raise ValueError(f"out must be a contiguous uint8 tensor of shape ({self.num_envs}, 32) on {self.device}")
+        with torch.cuda.device(self.device):
+            _lib.check(self._L.mg_hash(self._h, self._p(out), self._stream()))
+        return out
+
+    def hash(self, size: int = 16):
+        """[env.hash(size) for every env]: the reference's hex strings, 1 <= size <= 64 (synchronises)."""
+        if not 1 <= int(size) <= 64:
+            raise ValueError("size must be in 1..64 (a SHA-256 hex digest has 64 digits)")
+        d = self.hash_digest().cpu().numpy()
+        hexd = np.frombuffer(b"0123456789abcdef", np.uint8)
+        txt = np.empty((self.num_envs, 64), np.uint8)
+        txt[:, 0::2] = hexd[d >> 4]
+        txt[:, 1::2] = hexd[d & 15]
+        return np.ascontiguousarray(txt[:, :int(size)]).view(f"S{int(size)}").ravel().astype(str).tolist()
+
     def get_state(self):
         n, d = self.num_envs, self.device
         st = {
