@@ -58,7 +58,11 @@ extern "C" {
                                    obstructedmaze.py, obstructedmaze_v1.py: params {variant (0 Unlock, 1 UnlockPickup,
                                    2 BlockedUnlockPickup, 3 KeyCorridor, 4 ObstructedMaze_1Dlhb, 5 ObstructedMaze_Full,
                                    6 ObstructedMaze_Full_V1), room_size, num_rows, num_cols[, key_in_box, blocked,
-                                   agent_room_i | agent_room_j << 4, num_quarters]} */
+                                   agent_room_i | agent_room_j << 4, num_quarters]};
+                                   envs/babyai/goto.py, the one-room GoTo levels: {7, room_size 4..8, 1, 1, level
+                                   (0 GoToRedBallGrey, 1 GoToRedBall, 2 GoToObj, 3 GoToLocal, 4 GoToRedBlueBall), num_dists}
+                                   with at most 8 objects that the room can hold away from the agent; max_steps is
+                                   room_size^2 for the registered ids */
 #define MG_KIND_DYNOBS 15       /* envs/dynamicobstacles.py: params {n_obstacles, random_start, start_x, start_y, start_dir} */
 
 /* gymnasium.vector.AutoresetMode */

@@ -141,14 +141,26 @@ int mg_create(int kind, int width, int height, int max_steps, int see_through_wa
   if (kind == MG_KIND_MEMORY && (height % 2 == 0 || height < 7 || width < 7))
     return fail(MG_ERR_INVALID_ARG, "memory needs an odd height and at least 7 x 7 (memory.py:98)");
   if (kind == MG_KIND_ROOMGRID) {
-    if (n_params < 4 || params[0] < 0 || params[0] > 6 || params[1] < 3 || params[1] > 8 || params[2] < 1 || params[3] < 1 ||
+    if (n_params < 4 || params[0] < 0 || params[0] > RG_BABYAI_GOTO || params[1] < 3 || params[1] > 8 || params[2] < 1 || params[3] < 1 ||
         params[2] * params[3] > 9 || width != (params[1] - 1) * params[3] + 1 || height != (params[1] - 1) * params[2] + 1)
-      return fail(MG_ERR_INVALID_ARG, "roomgrid needs params {variant 0..3, room_size 3..8, num_rows, num_cols} with at most 9 rooms, "
+      return fail(MG_ERR_INVALID_ARG, "roomgrid needs params {variant 0..7, room_size 3..8, num_rows, num_cols} with at most 9 rooms, "
                                       "width = (room_size - 1) num_cols + 1 and height = (room_size - 1) num_rows + 1 (roomgrid.py:83-84)");
     if (params[0] == 3 && params[3] != 3) return fail(MG_ERR_INVALID_ARG, "keycorridor has 3 columns of rooms (keycorridor.py:104-126)");
     if (params[0] != 3 && params[0] < 5 && (params[2] != 1 || params[3] != 2))
       return fail(MG_ERR_INVALID_ARG, "unlock / unlockpickup / blockedunlockpickup / obstructedmaze-1D are 1 x 2 rooms");
-    if (params[0] >= 4) {
+    if (params[0] == RG_BABYAI_GOTO) {
+      // every object must find a cell: an interior cell that is free, not the agent's and not next to it. With the
+      // agent in the middle of a room of size S that leaves (S - 2)^2 - 5 cells; S = 4 has only corners, so 1 cell.
+      const int S = params[1], level = n_params >= 6 ? params[4] : -1, nd = n_params >= 6 ? params[5] : -1;
+      const int nobj = nd + ((level == BABYAI_OBJ || level == BABYAI_LOCAL) ? 0 : 1);
+      const int cap = S == 4 ? 1 : (S - 2) * (S - 2) - 5;
+      if (n_params < 6 || params[2] != 1 || params[3] != 1 || S < 4 || level < 0 || level > BABYAI_REDBLUEBALL || nd < 0 ||
+          (level == BABYAI_OBJ && nd != 1) || (level == BABYAI_LOCAL && nd < 1) || nobj > 8 || nobj > cap)
+        return fail(MG_ERR_INVALID_ARG, "babyai goto needs params {7, room_size 4..8, 1, 1, level 0..4 (GoToRedBallGrey, GoToRedBall, "
+                                        "GoToObj, GoToLocal, GoToRedBlueBall), num_dists}: one room, num_dists 1 for GoToObj and >= 1 for "
+                                        "GoToLocal, at most 8 objects and no more than the room has cells away from the agent");
+    }
+    if (rg_obstructed(params[0])) {
       if (n_params < 8 || params[1] < 4) return fail(MG_ERR_INVALID_ARG, "obstructedmaze needs params {variant, room_size >= 4, num_rows, num_cols, key_in_box, blocked, agent_room_i | agent_room_j << 4, num_quarters}");
       if (params[0] >= 5 && (params[2] != 3 || params[3] != 3 || params[7] < 1 || params[7] > 4 || (params[6] & 15) > 2 || (params[6] >> 4) > 2))
         return fail(MG_ERR_INVALID_ARG, "obstructedmaze-Full is 3 x 3 rooms with 1..4 quarters and the agent's room inside the grid");

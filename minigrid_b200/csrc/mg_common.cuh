@@ -80,7 +80,12 @@ constexpr int KIND_COUNT = 17;
 // kp[0] of KIND_ROOMGRID; the ObstructedMaze variants (envs/obstructedmaze.py, obstructedmaze_v1.py) also read
 // kp[4] key_in_box, kp[5] blocked, kp[6] agent room i | j << 4, kp[7] num_quarters
 enum : int { RG_UNLOCK = 0, RG_UNLOCKPICKUP = 1, RG_BLOCKEDUNLOCKPICKUP = 2, RG_KEYCORRIDOR = 3, RG_OBSTRUCTED_1D = 4,
-             RG_OBSTRUCTED_FULL = 5, RG_OBSTRUCTED_FULL_V1 = 6 };  // kinds mg_create accepts: the kernels are instantiated for the kinds below this
+             RG_OBSTRUCTED_FULL = 5, RG_OBSTRUCTED_FULL_V1 = 6,
+             // the single-room BabyAI GoTo levels (envs/babyai/goto.py): kp = {7, room_size, 1, 1, level, num_dists}
+             RG_BABYAI_GOTO = 7 };  // kinds mg_create accepts: the kernels are instantiated for the kinds below this
+MG_HD bool rg_obstructed(int variant) { return variant >= RG_OBSTRUCTED_1D && variant <= RG_OBSTRUCTED_FULL_V1; }
+// kp[4] of RG_BABYAI_GOTO: GoToRedBallGrey, GoToRedBall(NoDists), GoToObj, GoToLocal, GoToRedBlueBall
+enum : int { BABYAI_REDBALL_GREY = 0, BABYAI_REDBALL = 1, BABYAI_OBJ = 2, BABYAI_LOCAL = 3, BABYAI_REDBLUEBALL = 4 };
 enum : int { AUTORESET_NEXT_STEP = 0, AUTORESET_SAME_STEP = 1, AUTORESET_DISABLED = 2 };
 // bits of the sticky device error word (Params::err)
 enum : int { ERR_BAD_ACTION = 1, ERR_BAD_STATE = 2, ERR_PACKED_RANGE = 4 };

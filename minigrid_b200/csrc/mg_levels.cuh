@@ -270,7 +270,7 @@ MG_D uint32_t cell_roomgrid(const Geom &g, const int *kp, const Level &L, int x,
     const uint32_t dsc = rg_hdoor(L, (j - 1) * cols + i);
     return ((dsc & 0x80u) && lx - 1 == (int)(dsc & 7u)) ? rg_door_code(dsc) : CODE_WALL;
   }
-  if (kp[0] >= RG_OBSTRUCTED_1D && x == L.e && y == L.f) return T_BALL | (C_BLUE << 4);  // self.obj: COLOR_NAMES[0]
+  if (rg_obstructed(kp[0]) && x == L.e && y == L.f) return T_BALL | (C_BLUE << 4);  // self.obj: COLOR_NAMES[0]
   // the objects in creation order; a later grid.set wins (ObstructedMaze v0 puts blocking balls over earlier keys)
   for (int k = 15; k >= 0; --k)
     if (k < L.nrooms) {
@@ -479,7 +479,55 @@ MG_D void draw_level(const Params &p, Pcg &r, Level &L) {
       }
     };
     int dpx = 0, dpy = 0;
-    if (variant >= RG_OBSTRUCTED_1D) {
+    if (variant == RG_BABYAI_GOTO) {
+      // RoomGridLevel._gen_grid (babyai/core/roomgrid_level.py:119-144): an attempt is RoomGrid._gen_grid (one room: no
+      // door draws) and gen_mission (babyai/goto.py:67-78, 133-141, 192-193, 256-260, 333-338, 661-677); RejectSampling
+      // starts the next attempt from an empty grid while the stream continues. The RecursionError of place_obj's 1000
+      // tries is not modelled: the worst case, GoToObjS4, has 1 valid cell in the 16 drawn, (15/16)^1001 ~ 1e-28.
+      const int level = p.kp[4], ndist = p.kp[5];
+      uint32_t tgt;
+      for (;;) {
+        L.rm03 = 0; L.nrooms = 0;
+        L.ax = S / 2; L.ay = S / 2; L.adir = 0;
+        place_agent(0, 0);  // place_agent(): i = _rand_int(0, 1), j = _rand_int(0, 1) draw nothing
+        tgt = 0;
+        if (level == BABYAI_REDBALL_GREY || level == BABYAI_REDBALL) tgt = add_object(0, 0, 1, C_RED);
+        bool red_or_blue_ball = false;
+        for (int k = 0; k < ndist; ++k) {  // add_distractors (roomgrid.py:396-438): colour, then type; all_unique only
+          const int col = (int)color_name_idx(rng_integers(r, 0, 6));  // matters for GoToObj, whose list starts empty
+          const int kind = rng_integers(r, 0, 3);
+          red_or_blue_ball |= kind == 1 && (col == (int)C_RED || col == (int)C_BLUE);
+          // GoToRedBallGrey recolours its distractors after placing them; placement does not look at colours
+          add_object(0, 0, kind, level == BABYAI_REDBALL_GREY ? (int)C_GREY : col);
+        }
+        if (level == BABYAI_OBJ) { tgt = rg_obj(L, 0); break; }  // no reachability check
+        if (level == BABYAI_REDBLUEBALL) {
+          if (red_or_blue_ball) continue;  // RejectSampling("can only have one blue or red ball")
+          tgt = add_object(0, 0, 1, rng_integers(r, 0, 2) == 0 ? (int)C_RED : (int)C_BLUE);
+        }
+        // check_objs_reachable (roomgrid_level.py:250-302): flood fill from the agent through empty cells; an object
+        // cell is reached but stops the fill; one unreached object rejects the attempt. The one room is the whole grid,
+        // <= 8 x 8 cells: bit y W + x of a 64-bit mask (border cells are walls, so no shift leaves the grid).
+        unsigned long long objs = 0, free = 0;
+        for (int y = 1; y < H - 1; ++y) free |= (((1ull << (W - 2)) - 1ull) << 1) << (y * W);
+        for (int k = 0; k < L.nrooms; ++k) {
+          const uint32_t o = rg_obj(L, k);
+          objs |= 1ull << ((int)((o >> 5) & 31u) * W + (int)(o & 31u));
+        }
+        free &= ~objs;
+        unsigned long long reach = 1ull << (L.ay * W + L.ax), prev = 0;
+        while (reach != prev) {
+          prev = reach;
+          const unsigned long long from = reach & free;
+          reach |= ((from << 1) | (from >> 1) | (from << W) | (from >> W)) & (free | objs);
+        }
+        if (objs & ~reach) continue;  // RejectSampling("unreachable object at ...")
+        if (level == BABYAI_LOCAL) tgt = rg_obj(L, rng_integers(r, 0, L.nrooms));  // _rand_elem(objs)
+        break;
+      }
+      // GoToInstr(ObjDesc(type, colour)): the step post-filter compares the front cell with (type, colour)
+      level_target(L, (int)(T_KEY + ((tgt >> 10) & 3u)), (int)((tgt >> 12) & 7u), 0u);
+    } else if (rg_obstructed(variant)) {
       // ObstructedMazeEnv._gen_grid (obstructedmaze.py:112-126): door_colors = _rand_subset(COLOR_NAMES, 6), the ball to find
       // is COLOR_NAMES[0] (blue), blocking balls COLOR_NAMES[1] (green), boxes COLOR_NAMES[2] (grey)
       const int key_in_box = p.kp[4], blocked = p.kp[5];

@@ -29,6 +29,8 @@ struct PostIn {
   // roomgrid only: kp[0], and whether the cell at (tx, ty) is an open door after the transition (Unlock's self.door.is_open)
   int variant;
   bool door_open;
+  // roomgrid BabyAI GoTo only: the code of the cell in front of the agent after the transition (0 = not read)
+  uint32_t front = 0;
 };
 enum : int { POST_KEEP = 0, POST_REWARD = 1, POST_ZERO = 2 };  // what becomes of the step's reward
 struct PostOut { uint32_t terminated; int reward; };
@@ -61,7 +63,13 @@ MG_HD PostOut post_filter(const PostIn &in, uint32_t terminated) {
     if (in.ax == in.tx && in.ay == in.ty) { o.reward = POST_REWARD; o.terminated = 1u; }
     if (in.ax == (int)(in.aux & 255u) && in.ay == (int)((in.aux >> 8) & 255u)) { o.reward = POST_ZERO; o.terminated = 1u; }
   } else if (KIND == KIND_ROOMGRID) {
-    if (in.variant == RG_UNLOCK) {  // unlock.py:88-96
+    if (in.variant == RG_BABYAI_GOTO) {
+      // RoomGridLevel.step (babyai/core/roomgrid_level.py:87-104) with GoToInstr.verify_action (verifier.py:290-316):
+      // success when front_pos is one of the positions find_matching_objs recorded at reset. A matching object leaves
+      // its cell only by being picked up, which needs the agent to face it first, and facing it already ended the
+      // episode; so the test is "the front cell holds an object of the target's type and colour" (tx, ty).
+      if ((int)(in.front & 15u) == in.tx && (int)((in.front >> 4) & 7u) == in.ty) { o.reward = POST_REWARD; o.terminated = 1u; }
+    } else if (in.variant == RG_UNLOCK) {  // unlock.py:88-96
       if (in.action == A_TOGGLE && in.door_open) { o.reward = POST_REWARD; o.terminated = 1u; }
     } else if (in.action == A_PICKUP && in.carry != 0u && (int)(in.carry & 15u) == in.tx && (int)((in.carry >> 4) & 7u) == in.ty) {
       // "self.carrying and self.carrying == self.obj" (unlockpickup.py:97-105, blockedunlockpickup.py:107-115,

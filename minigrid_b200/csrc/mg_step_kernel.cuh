@@ -565,7 +565,15 @@ k_step(const __grid_constant__ Params p, const void *__restrict__ actions, int a
         in.carry_before = carry_before; in.carry = carry;
         in.tx = tx; in.ty = ty; in.aux = flags >> 8;
         in.red_before = in.blue_before = in.red_after = in.blue_after = false;
-        in.variant = p.kp[0]; in.door_open = false;
+        in.variant = p.kp[0]; in.door_open = false; in.front = 0;
+        if (KIND == KIND_ROOMGRID && p.kp[0] == RG_BABYAI_GOTO) {  // the front cell after this step's turn, move or mutation
+          if (WIN) {  // the loaded words hold the agent's line for its new direction, the mutation included
+            in.front = view_words_byte(vw, ((dir & 1) ? ay : ax) + ((dir < 2) ? 1 : -1));
+          } else {
+            const int nx = ax + (dir == 0) - (dir == 2), ny = ay + (dir == 1) - (dir == 3);
+            in.front = (tile_word<true>(base, r_word(g, nx, ny)) >> (8 * (nx & 3))) & 0xFFu;
+          }
+        }
         if (KIND == KIND_ROOMGRID && p.kp[0] == RG_UNLOCK) {  // self.door.is_open: the cell at the target, after this step's mutation
           uint32_t cd;
           if (!WIN) cd = (tile_word<true>(base, r_word(g, tx, ty)) >> (8 * (tx & 3))) & 0xFFu;

@@ -232,8 +232,38 @@ REGISTRY = {
 }
 
 
+BABYAI_GOTO = 7  # roomgrid variant of the one-room BabyAI GoTo levels
+BABYAI_REDBALL_GREY, BABYAI_REDBALL, BABYAI_OBJ, BABYAI_LOCAL, BABYAI_REDBLUEBALL = 0, 1, 2, 3, 4
+
+
+def babyai_goto(level, room_size=8, num_dists=7, mission="go to {article} {color} {type}"):
+    """envs/babyai/goto.py on one room (babyai/core/roomgrid_level.py:46-85): max_steps = room_size^2 (one navigation).
+    The mission names the drawn target, and says "a" instead of "the" when several objects match it; a constant string
+    only where the level makes it one."""
+    return roomgrid(BABYAI_GOTO, room_size, 1, 1, room_size * room_size, mission, (level, num_dists))
+
+
+# __init__.py:573-665 (the BabyAI GoTo levels that fit in one room)
+BABYAI_REGISTRY = {
+    "BabyAI-GoToRedBallGrey-v0": babyai_goto(BABYAI_REDBALL_GREY, mission="go to the red ball"),
+    "BabyAI-GoToRedBall-v0": babyai_goto(BABYAI_REDBALL, mission="go to {article} red ball"),
+    "BabyAI-GoToRedBallNoDists-v0": babyai_goto(BABYAI_REDBALL, num_dists=0, mission="go to the red ball"),
+    "BabyAI-GoToObj-v0": babyai_goto(BABYAI_OBJ, num_dists=1, mission="go to the {color} {type}"),
+    "BabyAI-GoToObjS4-v0": babyai_goto(BABYAI_OBJ, 4, 1, "go to the {color} {type}"),
+    "BabyAI-GoToObjS6-v1": babyai_goto(BABYAI_OBJ, 6, 1, "go to the {color} {type}"),
+    "BabyAI-GoToLocal-v0": babyai_goto(BABYAI_LOCAL, num_dists=8),
+    **{f"BabyAI-GoToLocalS{s}N{n}-v0": babyai_goto(BABYAI_LOCAL, s, n)
+       for s, n in [(5, 2), (6, 2), (6, 3), (6, 4), (7, 4), (7, 5), (8, 2), (8, 3), (8, 4), (8, 5), (8, 6), (8, 7)]},
+    # the distractors are never red or blue balls, so the target is the only match
+    "BabyAI-GoToRedBlueBall-v0": babyai_goto(BABYAI_REDBLUEBALL, mission="go to the {color} ball"),
+}
+
+
 def get(env_id: str) -> EnvSpec:
+    if env_id in BABYAI_REGISTRY:
+        return BABYAI_REGISTRY[env_id]
     try:
         return REGISTRY[env_id]
     except KeyError:
-        raise KeyError(f"{env_id!r} is not one of the ids this engine implements: {sorted(REGISTRY)}") from None
+        raise KeyError(f"{env_id!r} is not one of the ids this engine implements: "
+                       f"{sorted(REGISTRY) + sorted(BABYAI_REGISTRY)}") from None
