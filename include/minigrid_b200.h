@@ -117,7 +117,9 @@ int mg_reset_masked(mg_env *env, const uint8_t *mask_dev, uint8_t *obs_dev, int3
 /* Replaces: MiniGridEnv.step(action) (minigrid_env.py:525-595) + gen_obs (:597-650) for every env, with
  * gymnasium.vector.SyncVectorEnv autoreset semantics (mode given at mg_create).
  * actions_dev: n actions of dtype action_dtype; obs_dev uint8[n][7][7][3]; dir_dev int32[n];
- * reward_dev float64[n]; terminated_dev / truncated_dev uint8[n] (0/1). */
+ * reward_dev float64[n]; terminated_dev / truncated_dev uint8[n] (0/1). The output pointers need no alignment beyond
+ * their element type's: obs_dev may start at any byte (e.g. step t of a rollout buffer, rollout_obs + t * n * 147); a
+ * 16-byte aligned obs_dev lets full tiles leave through one bulk store, any other goes through a byte copy. */
 int mg_step(mg_env *env, const void *actions_dev, int action_dtype, uint8_t *obs_dev, int32_t *dir_dev,
             double *reward_dev, uint8_t *terminated_dev, uint8_t *truncated_dev, void *stream);
 
