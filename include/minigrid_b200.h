@@ -62,7 +62,13 @@ extern "C" {
                                    envs/babyai/goto.py, the one-room GoTo levels: {7, room_size 4..8, 1, 1, level
                                    (0 GoToRedBallGrey, 1 GoToRedBall, 2 GoToObj, 3 GoToLocal, 4 GoToRedBlueBall), num_dists}
                                    with at most 8 objects that the room can hold away from the agent; max_steps is
-                                   room_size^2 for the registered ids */
+                                   room_size^2 for the registered ids;
+                                   envs/babyai/other.py (OneRoomS*), pickup.py (PickupDist), putnext.py (PutNextLocal):
+                                   {8, room_size, 1, 1, level (0 OneRoom, 1 PickupDist, 2 PutNextLocal), num_objs, strict}
+                                   with room_size 4..20 for OneRoom and 4..8 otherwise, num_objs 1 for OneRoom and >= 2 for
+                                   PutNextLocal, the same object capacity as GoTo, and strict (PickupInstr's) only on
+                                   PickupDist; max_steps is room_size^2 (OneRoom, PickupDist) or 2 room_size^2 (PutNextLocal)
+                                   for the registered ids */
 #define MG_KIND_DYNOBS 15       /* envs/dynamicobstacles.py: params {n_obstacles, random_start, start_x, start_y, start_dir} */
 
 /* gymnasium.vector.AutoresetMode */

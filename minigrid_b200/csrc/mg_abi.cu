@@ -141,10 +141,14 @@ int mg_create(int kind, int width, int height, int max_steps, int see_through_wa
   if (kind == MG_KIND_MEMORY && (height % 2 == 0 || height < 7 || width < 7))
     return fail(MG_ERR_INVALID_ARG, "memory needs an odd height and at least 7 x 7 (memory.py:98)");
   if (kind == MG_KIND_ROOMGRID) {
-    if (n_params < 4 || params[0] < 0 || params[0] > RG_BABYAI_GOTO || params[1] < 3 || params[1] > 8 || params[2] < 1 || params[3] < 1 ||
-        params[2] * params[3] > 9 || width != (params[1] - 1) * params[3] + 1 || height != (params[1] - 1) * params[2] + 1)
-      return fail(MG_ERR_INVALID_ARG, "roomgrid needs params {variant 0..7, room_size 3..8, num_rows, num_cols} with at most 9 rooms, "
-                                      "width = (room_size - 1) num_cols + 1 and height = (room_size - 1) num_rows + 1 (roomgrid.py:83-84)");
+    // BabyAI OneRoom is the one level whose room may be larger than 8: it has no reachability fill (a 64-bit mask)
+    const bool one_room = n_params >= 5 && params[0] == RG_BABYAI_PICKUP_PUTNEXT && params[4] == BABYAI_ONEROOM;
+    if (n_params < 4 || params[0] < 0 || params[0] > RG_BABYAI_PICKUP_PUTNEXT || params[1] < 3 || params[1] > (one_room ? 20 : 8) ||
+        params[2] < 1 || params[3] < 1 || params[2] * params[3] > 9 || width != (params[1] - 1) * params[3] + 1 ||
+        height != (params[1] - 1) * params[2] + 1)
+      return fail(MG_ERR_INVALID_ARG, "roomgrid needs params {variant 0..8, room_size 3..8 (..20 for BabyAI OneRoom), num_rows, num_cols} "
+                                      "with at most 9 rooms, width = (room_size - 1) num_cols + 1 and height = (room_size - 1) num_rows + 1 "
+                                      "(roomgrid.py:83-84)");
     if (params[0] == 3 && params[3] != 3) return fail(MG_ERR_INVALID_ARG, "keycorridor has 3 columns of rooms (keycorridor.py:104-126)");
     if (params[0] != 3 && params[0] < 5 && (params[2] != 1 || params[3] != 2))
       return fail(MG_ERR_INVALID_ARG, "unlock / unlockpickup / blockedunlockpickup / obstructedmaze-1D are 1 x 2 rooms");
@@ -159,6 +163,18 @@ int mg_create(int kind, int width, int height, int max_steps, int see_through_wa
         return fail(MG_ERR_INVALID_ARG, "babyai goto needs params {7, room_size 4..8, 1, 1, level 0..4 (GoToRedBallGrey, GoToRedBall, "
                                         "GoToObj, GoToLocal, GoToRedBlueBall), num_dists}: one room, num_dists 1 for GoToObj and >= 1 for "
                                         "GoToLocal, at most 8 objects and no more than the room has cells away from the agent");
+    }
+    if (params[0] == RG_BABYAI_PICKUP_PUTNEXT) {
+      // the same capacity rule as GoTo; OneRoom places one ball, PickupDist and PutNextLocal num_objs unique objects
+      const int S = params[1], level = n_params >= 7 ? params[4] : -1, nobj = n_params >= 7 ? params[5] : -1;
+      const int strict = n_params >= 7 ? params[6] : -1, cap = S == 4 ? 1 : (S - 2) * (S - 2) - 5;
+      if (n_params < 7 || params[2] != 1 || params[3] != 1 || S < 4 || level < 0 || level > BABYAI_PUTNEXTLOCAL ||
+          (level == BABYAI_ONEROOM && nobj != 1) || (level == BABYAI_PICKUPDIST && nobj < 1) || (level == BABYAI_PUTNEXTLOCAL && nobj < 2) ||
+          nobj > 8 || nobj > cap || strict < 0 || strict > 1 || (strict && level != BABYAI_PICKUPDIST))
+        return fail(MG_ERR_INVALID_ARG, "babyai pickup / putnext needs params {8, room_size, 1, 1, level 0..2 (OneRoom, PickupDist, "
+                                        "PutNextLocal), num_objs, strict}: one room, room_size 4..20 for OneRoom and 4..8 otherwise, "
+                                        "num_objs 1 for OneRoom and >= 2 for PutNextLocal, at most 8 objects and no more than the "
+                                        "room has cells away from the agent, strict 0 or 1 and 1 only for PickupDist");
     }
     if (rg_obstructed(params[0])) {
       if (n_params < 8 || params[1] < 4) return fail(MG_ERR_INVALID_ARG, "obstructedmaze needs params {variant, room_size >= 4, num_rows, num_cols, key_in_box, blocked, agent_room_i | agent_room_j << 4, num_quarters}");

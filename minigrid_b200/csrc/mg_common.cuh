@@ -82,10 +82,17 @@ constexpr int KIND_COUNT = 17;
 enum : int { RG_UNLOCK = 0, RG_UNLOCKPICKUP = 1, RG_BLOCKEDUNLOCKPICKUP = 2, RG_KEYCORRIDOR = 3, RG_OBSTRUCTED_1D = 4,
              RG_OBSTRUCTED_FULL = 5, RG_OBSTRUCTED_FULL_V1 = 6,
              // the single-room BabyAI GoTo levels (envs/babyai/goto.py): kp = {7, room_size, 1, 1, level, num_dists}
-             RG_BABYAI_GOTO = 7 };  // kinds mg_create accepts: the kernels are instantiated for the kinds below this
+             RG_BABYAI_GOTO = 7,
+             // the single-room BabyAI Pickup and PutNext levels (envs/babyai/other.py, pickup.py, putnext.py):
+             // kp = {8, room_size, 1, 1, level, num_objs, strict}
+             RG_BABYAI_PICKUP_PUTNEXT = 8 };  // kinds mg_create accepts: the kernels are instantiated for the kinds below this
 MG_HD bool rg_obstructed(int variant) { return variant >= RG_OBSTRUCTED_1D && variant <= RG_OBSTRUCTED_FULL_V1; }
 // kp[4] of RG_BABYAI_GOTO: GoToRedBallGrey, GoToRedBall(NoDists), GoToObj, GoToLocal, GoToRedBlueBall
 enum : int { BABYAI_REDBALL_GREY = 0, BABYAI_REDBALL = 1, BABYAI_OBJ = 2, BABYAI_LOCAL = 3, BABYAI_REDBLUEBALL = 4 };
+// kp[4] of RG_BABYAI_PICKUP_PUTNEXT: OneRoomS*, PickupDist(Debug), PutNextLocal*
+enum : int { BABYAI_ONEROOM = 0, BABYAI_PICKUPDIST = 1, BABYAI_PUTNEXTLOCAL = 2 };
+// level_aux of a Pickup level: which parts of ObjDesc(type, colour) are set, and PickupInstr's strict flag
+enum : uint32_t { PICK_TYPE = 1u, PICK_COLOR = 2u, PICK_STRICT = 4u };
 enum : int { AUTORESET_NEXT_STEP = 0, AUTORESET_SAME_STEP = 1, AUTORESET_DISABLED = 2 };
 // bits of the sticky device error word (Params::err)
 enum : int { ERR_BAD_ACTION = 1, ERR_BAD_STATE = 2, ERR_PACKED_RANGE = 4 };

@@ -478,8 +478,72 @@ MG_D void draw_level(const Params &p, Pcg &r, Level &L) {
         if (front == CODE_EMPTY || front == CODE_WALL) break;
       }
     };
+    // check_objs_reachable (roomgrid_level.py:250-302) on the BabyAI levels' one room: flood fill from the agent through
+    // empty cells; an object cell is reached but stops the fill; false when an object is not reached. The one room is
+    // the whole grid, <= 8 x 8 cells: bit y W + x of a 64-bit mask (border cells are walls, so no shift leaves the grid).
+    auto objs_reachable = [&]() -> bool {
+      unsigned long long objs = 0, free = 0;
+      for (int y = 1; y < H - 1; ++y) free |= (((1ull << (W - 2)) - 1ull) << 1) << (y * W);
+      for (int k = 0; k < L.nrooms; ++k) {
+        const uint32_t o = rg_obj(L, k);
+        objs |= 1ull << ((int)((o >> 5) & 31u) * W + (int)(o & 31u));
+      }
+      free &= ~objs;
+      unsigned long long reach = 1ull << (L.ay * W + L.ax), prev = 0;
+      while (reach != prev) {
+        prev = reach;
+        const unsigned long long from = reach & free;
+        reach |= ((from << 1) | (from >> 1) | (from << W) | (from >> W)) & (free | objs);
+      }
+      return !(objs & ~reach);
+    };
     int dpx = 0, dpy = 0;
-    if (variant == RG_BABYAI_GOTO) {
+    if (variant == RG_BABYAI_PICKUP_PUTNEXT) {
+      // RoomGridLevel._gen_grid (babyai/core/roomgrid_level.py:119-177) with the gen_mission of OneRoomS* (other.py:329-332),
+      // PickupDist (pickup.py:275-290) and PutNextLocal (putnext.py:71-80), then validate_instrs; RejectSampling starts
+      // the next attempt from an empty room while the stream continues. As for GoTo, place_obj's RecursionError is not
+      // modelled.
+      const int level = p.kp[4], nobj = p.kp[5];
+      uint32_t tx = 0, ty = 0, aux = 0;
+      for (;;) {
+        L.rm03 = 0; L.nrooms = 0;
+        L.ax = S / 2; L.ay = S / 2; L.adir = 0;
+        if (level == BABYAI_ONEROOM) {  // add_object(0, 0, kind="ball") draws the colour; PickupInstr(ObjDesc("ball"))
+          const uint32_t o = add_object(0, 0, 1, -1);
+          place_agent(0, 0);
+          tx = T_KEY + ((o >> 10) & 3u); ty = (o >> 12) & 7u; aux = PICK_TYPE;
+          break;
+        }
+        // PutNextLocal places the agent first; PickupDist's objects are placed around the default room centre
+        if (level == BABYAI_PUTNEXTLOCAL) place_agent(0, 0);
+        while (L.nrooms < nobj) {  // add_distractors(all_unique=True) (roomgrid.py:396-438): colour, then type
+          const uint32_t col = color_name_idx(rng_integers(r, 0, 6));
+          const uint32_t kind = (uint32_t)rng_integers(r, 0, 3);
+          bool dup = false;
+          for (int k = 0; k < L.nrooms; ++k) dup |= ((rg_obj(L, k) >> 10) & 31u) == (kind | (col << 2));
+          if (!dup) add_object(0, 0, (int)kind, (int)col);
+        }
+        if (level == BABYAI_PICKUPDIST) {
+          place_agent(0, 0);
+          const uint32_t o = rg_obj(L, rng_integers(r, 0, L.nrooms));  // _rand_elem(objs)
+          const int select_by = rng_integers(r, 0, 3);                // _rand_elem(["type", "color", "both"])
+          tx = T_KEY + ((o >> 10) & 3u); ty = (o >> 12) & 7u;
+          aux = (select_by == 1 ? 0u : PICK_TYPE) | (select_by == 0 ? 0u : PICK_COLOR) | (p.kp[6] ? PICK_STRICT : 0u);
+          break;
+        }
+        if (!objs_reachable()) continue;  // RejectSampling("unreachable object at ...")
+        // o1, o2 = _rand_subset(objs, 2): the second draw indexes the list without the first
+        const int i1 = rng_integers(r, 0, L.nrooms), i2 = rng_integers(r, 0, L.nrooms - 1);
+        const uint32_t mv = rg_obj(L, i1), fo = rg_obj(L, i2 < i1 ? i2 : i2 + 1);
+        const int ddx = (int)(mv & 31u) - (int)(fo & 31u), ddy = (int)((mv >> 5) & 31u) - (int)((fo >> 5) & 31u);
+        if ((ddx < 0 ? -ddx : ddx) + (ddy < 0 ? -ddy : ddy) == 1) continue;  // RejectSampling("objs already next to each other")
+        // PutNextInstr(ObjDesc(move), ObjDesc(fixed)): the move object's type and colour, the fixed object's cell code
+        tx = T_KEY + ((mv >> 10) & 3u); ty = (mv >> 12) & 7u;
+        aux = (T_KEY + ((fo >> 10) & 3u)) | (((fo >> 12) & 7u) << 4);
+        break;
+      }
+      level_target(L, (int)tx, (int)ty, aux);
+    } else if (variant == RG_BABYAI_GOTO) {
       // RoomGridLevel._gen_grid (babyai/core/roomgrid_level.py:119-144): an attempt is RoomGrid._gen_grid (one room: no
       // door draws) and gen_mission (babyai/goto.py:67-78, 133-141, 192-193, 256-260, 333-338, 661-677); RejectSampling
       // starts the next attempt from an empty grid while the stream continues. The RecursionError of place_obj's 1000
@@ -505,23 +569,7 @@ MG_D void draw_level(const Params &p, Pcg &r, Level &L) {
           if (red_or_blue_ball) continue;  // RejectSampling("can only have one blue or red ball")
           tgt = add_object(0, 0, 1, rng_integers(r, 0, 2) == 0 ? (int)C_RED : (int)C_BLUE);
         }
-        // check_objs_reachable (roomgrid_level.py:250-302): flood fill from the agent through empty cells; an object
-        // cell is reached but stops the fill; one unreached object rejects the attempt. The one room is the whole grid,
-        // <= 8 x 8 cells: bit y W + x of a 64-bit mask (border cells are walls, so no shift leaves the grid).
-        unsigned long long objs = 0, free = 0;
-        for (int y = 1; y < H - 1; ++y) free |= (((1ull << (W - 2)) - 1ull) << 1) << (y * W);
-        for (int k = 0; k < L.nrooms; ++k) {
-          const uint32_t o = rg_obj(L, k);
-          objs |= 1ull << ((int)((o >> 5) & 31u) * W + (int)(o & 31u));
-        }
-        free &= ~objs;
-        unsigned long long reach = 1ull << (L.ay * W + L.ax), prev = 0;
-        while (reach != prev) {
-          prev = reach;
-          const unsigned long long from = reach & free;
-          reach |= ((from << 1) | (from >> 1) | (from << W) | (from >> W)) & (free | objs);
-        }
-        if (objs & ~reach) continue;  // RejectSampling("unreachable object at ...")
+        if (!objs_reachable()) continue;  // RejectSampling("unreachable object at ...")
         if (level == BABYAI_LOCAL) tgt = rg_obj(L, rng_integers(r, 0, L.nrooms));  // _rand_elem(objs)
         break;
       }

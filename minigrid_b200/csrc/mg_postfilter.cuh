@@ -31,6 +31,10 @@ struct PostIn {
   bool door_open;
   // roomgrid BabyAI GoTo only: the code of the cell in front of the agent after the transition (0 = not read)
   uint32_t front = 0;
+  // roomgrid BabyAI Pickup / PutNext only: kp[4], and on a drop the codes of the three cells next to the front cell other
+  // than the agent's, one per byte, after the transition (0 = not read)
+  int level = 0;
+  uint32_t next_to = 0;
 };
 enum : int { POST_KEEP = 0, POST_REWARD = 1, POST_ZERO = 2 };  // what becomes of the step's reward
 struct PostOut { uint32_t terminated; int reward; };
@@ -69,6 +73,30 @@ MG_HD PostOut post_filter(const PostIn &in, uint32_t terminated) {
       // its cell only by being picked up, which needs the agent to face it first, and facing it already ended the
       // episode; so the test is "the front cell holds an object of the target's type and colour" (tx, ty).
       if ((int)(in.front & 15u) == in.tx && (int)((in.front >> 4) & 7u) == in.ty) { o.reward = POST_REWARD; o.terminated = 1u; }
+    } else if (in.variant == RG_BABYAI_PICKUP_PUTNEXT) {
+      // RoomGridLevel.step (babyai/core/roomgrid_level.py:87-104). The verifiers' preCarrying is what was carried after
+      // the previous step: carry_before. No object appears or changes colour in these rooms (a box can only vanish, by
+      // toggle), so "is one of obj_set" is "matches the descriptor", and an object is identified by its cell code.
+      if (in.level == BABYAI_PUTNEXTLOCAL) {
+        // PutNextInstr.verify_action (verifier.py:411-435) after update_objs_poss on a drop: success when preCarrying is
+        // the move object and its cur_pos is 4-adjacent to where the fixed object (cell code aux) is now. A drop that
+        // failed leaves cur_pos = (-1, -1) from the pickup; one that succeeded put it in the front cell, and the fixed
+        // object next to that cell is in one of the three neighbours that are not the agent's cell.
+        const uint32_t f = in.aux & 0xFFu, n = in.next_to;
+        const bool moved = (int)(in.carry_before & 15u) == in.tx && (int)((in.carry_before >> 4) & 7u) == in.ty;
+        if (in.action == A_DROP && in.carry == 0u && moved &&
+            ((n & 0xFFu) == f || ((n >> 8) & 0xFFu) == f || ((n >> 16) & 0xFFu) == f)) {
+          o.reward = POST_REWARD; o.terminated = 1u;
+        }
+      } else if (in.action == A_PICKUP) {
+        // PickupInstr.verify_action (verifier.py:343-363): success when nothing was carried and the carried object
+        // matches ObjDesc(type if PICK_TYPE, colour if PICK_COLOR); strict: any other pickup that leaves something
+        // carried (the wrong object, or pressing pickup while carrying) fails
+        const bool match = in.carry != 0u && (!(in.aux & PICK_TYPE) || (int)(in.carry & 15u) == in.tx) &&
+                           (!(in.aux & PICK_COLOR) || (int)((in.carry >> 4) & 7u) == in.ty);
+        if (in.carry_before == 0u && match) { o.reward = POST_REWARD; o.terminated = 1u; }
+        else if ((in.aux & PICK_STRICT) && in.carry != 0u) { o.reward = POST_ZERO; o.terminated = 1u; }
+      }
     } else if (in.variant == RG_UNLOCK) {  // unlock.py:88-96
       if (in.action == A_TOGGLE && in.door_open) { o.reward = POST_REWARD; o.terminated = 1u; }
     } else if (in.action == A_PICKUP && in.carry != 0u && (int)(in.carry & 15u) == in.tx && (int)((in.carry >> 4) & 7u) == in.ty) {

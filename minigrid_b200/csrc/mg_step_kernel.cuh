@@ -137,6 +137,18 @@ static __device__ __noinline__ WrapOut wrap_step(const Params &p, int env, bool 
   return o;
 }
 
+// PutNextLocal's post-filter input on a drop: the codes of the three cells next to the front cell (fx, fy) other than
+// the agent's (the one beyond it, then the two beside it), one per byte. A drop changes only the front cell and every
+// earlier change was written through to the grid arena, so they are read from there, out of line, behind a branch the
+// other kinds and variants never take. A cell outside the grid (a byte of another line or of the ring) is read only when the front
+// cell is a wall, where no drop succeeds and the filter does not look at them.
+static __device__ __noinline__ uint32_t putnext_neighbours(const Params &p, int env, int fx, int fy, int dir) {
+  const uint8_t *gb = reinterpret_cast<const uint8_t *>(p.grid);
+  const int ddx = (dir == 0) - (dir == 2), ddy = (dir == 1) - (dir == 3);
+  auto cell = [&](int x, int y) { return (uint32_t)gb[cell_byte_R(p.g, env, x, y)]; };
+  return cell(fx + ddx, fy + ddy) | (cell(fx - ddy, fy + ddx) << 8) | (cell(fx + ddy, fy - ddx) << 16);
+}
+
 // MiniGridEnv.reset() for the lanes in `pend`. Phase 1: every pending lane replays the numpy-exact draws of ITS
 // environment (lane per env; only the rejection loops diverge). Phase 2, one environment at a time with the whole
 // warp: the owner's drawn integers are broadcast, lane L copies words L, L+32, ... of the level template into HBM
@@ -574,6 +586,9 @@ k_step(const __grid_constant__ Params p, const void *__restrict__ actions, int a
             in.front = (tile_word<true>(base, r_word(g, nx, ny)) >> (8 * (nx & 3))) & 0xFFu;
           }
         }
+        in.level = p.kp[4]; in.next_to = 0;
+        if (KIND == KIND_ROOMGRID && p.kp[0] == RG_BABYAI_PICKUP_PUTNEXT && act == A_DROP)
+          in.next_to = putnext_neighbours(p, env, fx, fy, dir);
         if (KIND == KIND_ROOMGRID && p.kp[0] == RG_UNLOCK) {  // self.door.is_open: the cell at the target, after this step's mutation
           uint32_t cd;
           if (!WIN) cd = (tile_word<true>(base, r_word(g, tx, ty)) >> (8 * (tx & 3))) & 0xFFu;

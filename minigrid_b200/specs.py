@@ -259,11 +259,40 @@ BABYAI_REGISTRY = {
 }
 
 
+BABYAI_PICKUP_PUTNEXT = 8  # roomgrid variant of the one-room BabyAI Pickup and PutNext levels
+BABYAI_ONEROOM, BABYAI_PICKUPDIST, BABYAI_PUTNEXTLOCAL = 0, 1, 2
+
+
+def babyai_pickup_putnext(level, room_size, num_objs, num_navs, mission, strict=False):
+    """envs/babyai/other.py (OneRoomS*), pickup.py (PickupDist), putnext.py (PutNextLocal) on one room: max_steps =
+    num_navs * room_size^2 (roomgrid_level.py:71-85; PutNextInstr needs two navigations). PickupDist's mission drops the
+    colour or says "object" instead of the type, as its drawn descriptor does."""
+    return roomgrid(BABYAI_PICKUP_PUTNEXT, room_size, 1, 1, num_navs * room_size * room_size, mission,
+                    (level, num_objs, int(strict)))
+
+
+# __init__.py:864-873, 883-898, 1059-1081 (the BabyAI Pickup and PutNext levels that fit in one room)
+BABYAI_PICKUP_PUTNEXT_REGISTRY = {
+    **{f"BabyAI-OneRoomS{s}-v0": babyai_pickup_putnext(BABYAI_ONEROOM, s, 1, 1, "pick up the ball")
+       for s in (8, 12, 16, 20)},
+    "BabyAI-PickupDist-v0": babyai_pickup_putnext(BABYAI_PICKUPDIST, 7, 5, 1, "pick up {article} {color} {type}"),
+    "BabyAI-PickupDistDebug-v0": babyai_pickup_putnext(BABYAI_PICKUPDIST, 7, 5, 1, "pick up {article} {color} {type}",
+                                                       strict=True),
+    "BabyAI-PutNextLocal-v0": babyai_pickup_putnext(BABYAI_PUTNEXTLOCAL, 8, 8, 2,
+                                                    "put the {color} {type} next to the {color} {type}"),
+    **{f"BabyAI-PutNextLocalS{s}N{n}-v0": babyai_pickup_putnext(BABYAI_PUTNEXTLOCAL, s, n, 2,
+                                                                "put the {color} {type} next to the {color} {type}")
+       for s, n in [(5, 3), (6, 4)]},
+}
+
+
 def get(env_id: str) -> EnvSpec:
     if env_id in BABYAI_REGISTRY:
         return BABYAI_REGISTRY[env_id]
+    if env_id in BABYAI_PICKUP_PUTNEXT_REGISTRY:
+        return BABYAI_PICKUP_PUTNEXT_REGISTRY[env_id]
     try:
         return REGISTRY[env_id]
     except KeyError:
         raise KeyError(f"{env_id!r} is not one of the ids this engine implements: "
-                       f"{sorted(REGISTRY) + sorted(BABYAI_REGISTRY)}") from None
+                       f"{sorted(REGISTRY) + sorted(BABYAI_REGISTRY) + sorted(BABYAI_PICKUP_PUTNEXT_REGISTRY)}") from None

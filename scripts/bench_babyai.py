@@ -1,11 +1,12 @@
 """BabyAI GoTo env-steps/s on the GPU, and the cost of the BabyAI branch to the existing roomgrid kinds.
 
-    python scripts/bench_babyai.py [--parent DIR] [--repeats 3] [--steps 400]
+    python scripts/bench_babyai.py [--ids ID,...] [--parent DIR] [--ab-ids ID,...] [--repeats 3] [--steps 400]
 
 Runs `bench.py --env ID --no-configs --no-cpu-baseline` (262144 envs, desynchronised NEXT_STEP episodes, CUDA graphs)
-as a subprocess per measurement and prints one JSON line: the headline value of every BabyAI id in IDS, and, with
---parent pointing at a built checkout of an earlier revision, the A/B of the DoorKey-8x8 headline and of
-KeyCorridorS6R3 between that checkout and this one, the two alternated `--repeats` times. The GPU's name and power
+as a subprocess per measurement and prints one JSON line: the headline value of every BabyAI id in --ids (default IDS),
+and, with --parent pointing at a built checkout of an earlier revision, the A/B of every id in --ab-ids (default
+AB_IDS: the DoorKey-8x8 headline and KeyCorridorS6R3) between that checkout and this one, the two alternated
+`--repeats` times. The GPU's name and power
 limit are read in the same run. Writes nothing to the tree.
 """
 from __future__ import annotations
@@ -39,19 +40,22 @@ def gpu_info():
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--ids", default=",".join(IDS), help="comma-separated ids to measure")
     ap.add_argument("--parent", help="a built checkout of the revision to compare against")
+    ap.add_argument("--ab-ids", default=",".join(AB_IDS), help="comma-separated ids of the A/B against --parent")
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--steps", type=int, default=400)
     ap.add_argument("--warmup", type=int, default=50)
     args = ap.parse_args()
     res = {**gpu_info(), "envs": 262144, "steps": args.steps, "babyai": {}}
-    for env_id in IDS:
+    for env_id in args.ids.split(","):
         res["babyai"][env_id] = bench(ROOT, env_id, args.steps, args.warmup)
     if args.parent:
         args.parent = os.path.abspath(args.parent)
-        res["ab"] = {env_id: {"parent": [], "this": []} for env_id in AB_IDS}
+        ab_ids = args.ab_ids.split(",")
+        res["ab"] = {env_id: {"parent": [], "this": []} for env_id in ab_ids}
         for _ in range(args.repeats):
-            for env_id in AB_IDS:
+            for env_id in ab_ids:
                 for side, tree in (("parent", args.parent), ("this", ROOT)):
                     res["ab"][env_id][side].append(bench(tree, env_id, args.steps, args.warmup)["value"])
     print(json.dumps(res))
