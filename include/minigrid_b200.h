@@ -91,7 +91,8 @@ typedef struct mg_env mg_env;
  * params: EMPTY {random_start, start_x, start_y, start_dir}; CROSSING {num_crossings, obstacle_type
  * (9 lava | 2 wall)}; LAVAGAP {obstacle_type}; DISTSHIFT {strip2_row, start_x, start_y, start_dir};
  * MULTIROOM {minNumRooms, maxNumRooms, maxRoomSize}; others (DOORKEY, FOURROOMS, LOCKEDROOM, PLAYGROUND) none.
- * device < 0 selects the current CUDA device. */
+ * device < 0 selects the current CUDA device. Creating or destroying a handle never changes how another handle
+ * launches, whatever the two ids and sizes. */
 int mg_create(int kind, int width, int height, int max_steps, int see_through_walls,
               const int32_t *params, int n_params, int64_t n_envs, int autoreset_mode, int device,
               mg_env **out);

@@ -83,7 +83,8 @@ cudaError_t configure_hash(const Params &p, int *grid_out) {
   int dev = 0, sms = 0, ctas = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  // the attribute belongs to the kernel, not the handle: the largest geometry's need, so no handle lowers it for another
+  // the attribute belongs to the kernel, not the handle (as K1's, configure_step): the largest geometry's need, so no
+  // handle lowers it for another
   const size_t smem_max = hash_smem_bytes(make_geom(MAX_DIM, MAX_DIM, LAYOUT_TILED));
   if (e == cudaSuccess) e = cudaFuncSetAttribute(k_hash, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
   if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas, k_hash, HASH_WARPS * 32, smem);

@@ -47,6 +47,8 @@ static StepKernel step_kernel(int kind, int vis, int mode) {
 // is still 9-26 % faster for the last three and for GoToDoor, 2.5 % slower for Fetch (profiles/plan_sweep_h100.txt), so
 // the choice stays the same for every kind.
 // MINIGRID_B200_CFG="warps,vis,nbuf" (vis: 1 ALU, 2 table) overrides the choice (tuning knob).
+// The K1 kernels declare no static shared memory (ptxas -v), so the whole bound is dynamic.
+constexpr int K1_SMEM_MAX = 227 * 1024 - 1024;
 cudaError_t configure_step(const Params &p, StepPlan *plan) {
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
@@ -67,10 +69,11 @@ cudaError_t configure_step(const Params &p, StepPlan *plan) {
       const int wcap = (nbuf == 2 || win) ? 20 : 28;  // __launch_bounds__ of the variants
       int wmax = 0;
       for (int w = wcap; w >= 1; --w)
-        if (step_smem_bytes(p.g, vis, w, nbuf) <= 227 * 1024 - 1024) { wmax = w; break; }
+        if (step_smem_bytes(p.g, vis, w, nbuf) <= K1_SMEM_MAX) { wmax = w; break; }
       if (wmax == 0) continue;
-      cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           (int)step_smem_bytes(p.g, vis, wmax, nbuf));
+      // the attribute belongs to the kernel, not the handle, and every geometry shares one K1 per (kind, vis, mode):
+      // one bound for all of them, so that no handle lowers it below another's plan.smem
+      cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, K1_SMEM_MAX);
       if (e != cudaSuccess) return e;
       for (int w = wmax; w >= (want_warps ? 1 : (wmax + 1) / 2); --w) {
         if (want_warps && w != want_warps) continue;

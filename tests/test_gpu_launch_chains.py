@@ -650,17 +650,32 @@ def test_past_order_cap(env_id, layout, cfg, monkeypatch, capfd):
 
 
 # ---- 6. concurrent and interleaved handles ----
+PAIRS = {  # (env_id, layout, MINIGRID_B200_LAYOUT at its mg_create) in creation order
+    # two different K1 kernels
+    "doorkey-fourrooms": (("MiniGrid-DoorKey-8x8-v0", TILED, None), ("MiniGrid-FourRooms-v0", WINDOW, None)),
+    # one K1 kernel, two geometries, the larger plan created first: the second mg_create must leave the kernel able to
+    # launch the first handle's plan
+    "keycorridor-s4r3-s3r1": (("MiniGrid-KeyCorridorS4R3-v0", TILED, None), ("MiniGrid-KeyCorridorS3R1-v0", TILED, None)),
+    "doorkey-16x16-tiled-5x5": (("MiniGrid-DoorKey-16x16-v0", TILED, "0"), ("MiniGrid-DoorKey-5x5-v0", TILED, None)),
+}
+
+
 @pytest.mark.parametrize("mode", ["next_step", "same_step"])
 @pytest.mark.parametrize("streams", ["two-streams", "one-stream"])
-def test_two_handles(streams, mode, monkeypatch, capfd):
-    """DoorKey-8x8 and FourRooms chains enqueued alternately: on two streams (two K1 grids share the GPU) or on one
-    (the benchmark's rotation of batches)."""
+@pytest.mark.parametrize("pair", list(PAIRS))
+def test_two_handles(pair, streams, mode, monkeypatch, capfd):
+    """Chains of two handles enqueued alternately: on two streams (two K1 grids share the GPU) or on one (the
+    benchmark's rotation of batches). The pairs that share a K1 kernel are a training env and an eval env of another
+    size."""
     n, T = 20000, 32
-    case = f"two-handles/{streams}/{mode}"
-    ids = (("MiniGrid-DoorKey-8x8-v0", TILED), ("MiniGrid-FourRooms-v0", WINDOW))
+    case = f"two-handles/{pair}/{streams}/{mode}"
+    ids = PAIRS[pair]
     envs, orcs, acts, slots = [], [], [], []
-    for k, (env_id, layout) in enumerate(ids):
+    for k, (env_id, layout, force_layout) in enumerate(ids):
+        if force_layout is not None:
+            monkeypatch.setenv("MINIGRID_B200_LAYOUT", force_layout)
         env, plan = make_engine(env_id, n, mode, monkeypatch, capfd)
+        monkeypatch.delenv("MINIGRID_B200_LAYOUT", raising=False)
         check_plan(case, plan, env_id, n, layout)
         orc = make_oracle(env_id, n, mode)
         env.reset(seed=1200 + k)
