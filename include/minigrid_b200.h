@@ -68,7 +68,15 @@ extern "C" {
                                    with room_size 4..20 for OneRoom and 4..8 otherwise, num_objs 1 for OneRoom and >= 2 for
                                    PutNextLocal, the same object capacity as GoTo, and strict (PickupInstr's) only on
                                    PickupDist; max_steps is room_size^2 (OneRoom, PickupDist) or 2 room_size^2 (PutNextLocal)
-                                   for the registered ids */
+                                   for the registered ids;
+                                   envs/babyai/open.py (OpenRedDoor, OpenDoor*, OpenTwoDoors, OpenRedBlueDoors*,
+                                   OpenDoorsOrder*), unlock.py (UnlockLocal*): {9, room_size 5..8, num_rows, num_cols, level
+                                   (0 OpenRedDoor, 1 OpenDoor, 2 OpenTwoDoors, 3 OpenDoorsOrder, 4 UnlockLocal), arg, strict}
+                                   with 1 x 2 rooms for OpenRedDoor and 3 x 3 otherwise; arg is OpenDoor's select_by (0
+                                   colour, 1 loc, 2 drawn), OpenTwoDoors' fixed red / blue colours (0 or 1), OpenDoorsOrder's
+                                   num_doors (2..4) or UnlockLocal's distractors (0 or 1), 0 for OpenRedDoor; strict is the
+                                   Debug ids' flag (never on OpenRedDoor or UnlockLocal); max_steps is room_size^2 rows cols,
+                                   or 720 for OpenTwoDoors and OpenDoorsOrder, for the registered ids */
 #define MG_KIND_DYNOBS 15       /* envs/dynamicobstacles.py: params {n_obstacles, random_start, start_x, start_y, start_dir} */
 
 /* gymnasium.vector.AutoresetMode */

@@ -143,10 +143,10 @@ int mg_create(int kind, int width, int height, int max_steps, int see_through_wa
   if (kind == MG_KIND_ROOMGRID) {
     // BabyAI OneRoom is the one level whose room may be larger than 8: it has no reachability fill (a 64-bit mask)
     const bool one_room = n_params >= 5 && params[0] == RG_BABYAI_PICKUP_PUTNEXT && params[4] == BABYAI_ONEROOM;
-    if (n_params < 4 || params[0] < 0 || params[0] > RG_BABYAI_PICKUP_PUTNEXT || params[1] < 3 || params[1] > (one_room ? 20 : 8) ||
+    if (n_params < 4 || params[0] < 0 || params[0] > RG_BABYAI_OPEN || params[1] < 3 || params[1] > (one_room ? 20 : 8) ||
         params[2] < 1 || params[3] < 1 || params[2] * params[3] > 9 || width != (params[1] - 1) * params[3] + 1 ||
         height != (params[1] - 1) * params[2] + 1)
-      return fail(MG_ERR_INVALID_ARG, "roomgrid needs params {variant 0..8, room_size 3..8 (..20 for BabyAI OneRoom), num_rows, num_cols} "
+      return fail(MG_ERR_INVALID_ARG, "roomgrid needs params {variant 0..9, room_size 3..8 (..20 for BabyAI OneRoom), num_rows, num_cols} "
                                       "with at most 9 rooms, width = (room_size - 1) num_cols + 1 and height = (room_size - 1) num_rows + 1 "
                                       "(roomgrid.py:83-84)");
     if (params[0] == 3 && params[3] != 3) return fail(MG_ERR_INVALID_ARG, "keycorridor has 3 columns of rooms (keycorridor.py:104-126)");
@@ -175,6 +175,26 @@ int mg_create(int kind, int width, int height, int max_steps, int see_through_wa
                                         "PutNextLocal), num_objs, strict}: one room, room_size 4..20 for OneRoom and 4..8 otherwise, "
                                         "num_objs 1 for OneRoom and >= 2 for PutNextLocal, at most 8 objects and no more than the "
                                         "room has cells away from the agent, strict 0 or 1 and 1 only for PickupDist");
+    }
+    if (params[0] == RG_BABYAI_OPEN) {
+      // a door needs a neighbouring room (roomgrid.py:268-270): OpenRedDoor's is right of room (0, 0) in 1 x 2 rooms, the
+      // others are room (1, 1)'s in 3 x 3 rooms. A room of 5 still holds UnlockLocalDist's four objects away from the
+      // agent's default cell.
+      const int level = n_params >= 7 ? params[4] : -1, arg = n_params >= 7 ? params[5] : -1;
+      const int strict = n_params >= 7 ? params[6] : -1;
+      const bool rooms = level == BABYAI_OPENREDDOOR ? (params[2] == 1 && params[3] == 2) : (params[2] == 3 && params[3] == 3);
+      const bool flags = level == BABYAI_OPENREDDOOR ? (arg == 0 && strict == 0)
+                         : level == BABYAI_OPENDOOR ? (arg >= 0 && arg <= 2 && (strict == 0 || strict == 1))
+                         : level == BABYAI_OPENTWODOORS ? ((arg == 0 || arg == 1) && (strict == 0 || strict == 1))
+                         : level == BABYAI_OPENDOORSORDER ? (arg >= 2 && arg <= 4 && (strict == 0 || strict == 1))
+                         : level == BABYAI_UNLOCKLOCAL && (arg == 0 || arg == 1) && strict == 0;
+      if (n_params < 7 || params[1] < 5 || !rooms || !flags)
+        return fail(MG_ERR_INVALID_ARG, "babyai open needs params {9, room_size 5..8, num_rows, num_cols, level 0..4 (OpenRedDoor, "
+                                        "OpenDoor, OpenTwoDoors, OpenDoorsOrder, UnlockLocal), arg, strict}: 1 x 2 rooms for "
+                                        "OpenRedDoor and 3 x 3 otherwise; arg is select_by 0..2 (colour, loc, drawn) for OpenDoor, "
+                                        "fixed red / blue 0 or 1 for OpenTwoDoors, num_doors 2..4 for OpenDoorsOrder and "
+                                        "distractors 0 or 1 for UnlockLocal (0 for OpenRedDoor); strict 0 or 1, and 0 for "
+                                        "OpenRedDoor and UnlockLocal");
     }
     if (rg_obstructed(params[0])) {
       if (n_params < 8 || params[1] < 4) return fail(MG_ERR_INVALID_ARG, "obstructedmaze needs params {variant, room_size >= 4, num_rows, num_cols, key_in_box, blocked, agent_room_i | agent_room_j << 4, num_quarters}");

@@ -85,7 +85,10 @@ enum : int { RG_UNLOCK = 0, RG_UNLOCKPICKUP = 1, RG_BLOCKEDUNLOCKPICKUP = 2, RG_
              RG_BABYAI_GOTO = 7,
              // the single-room BabyAI Pickup and PutNext levels (envs/babyai/other.py, pickup.py, putnext.py):
              // kp = {8, room_size, 1, 1, level, num_objs, strict}
-             RG_BABYAI_PICKUP_PUTNEXT = 8 };  // kinds mg_create accepts: the kernels are instantiated for the kinds below this
+             RG_BABYAI_PICKUP_PUTNEXT = 8,
+             // the BabyAI Open and UnlockLocal levels (envs/babyai/open.py, unlock.py):
+             // kp = {9, room_size, num_rows, num_cols, level, arg, strict}
+             RG_BABYAI_OPEN = 9 };  // kinds mg_create accepts: the kernels are instantiated for the kinds below this
 MG_HD bool rg_obstructed(int variant) { return variant >= RG_OBSTRUCTED_1D && variant <= RG_OBSTRUCTED_FULL_V1; }
 // kp[4] of RG_BABYAI_GOTO: GoToRedBallGrey, GoToRedBall(NoDists), GoToObj, GoToLocal, GoToRedBlueBall
 enum : int { BABYAI_REDBALL_GREY = 0, BABYAI_REDBALL = 1, BABYAI_OBJ = 2, BABYAI_LOCAL = 3, BABYAI_REDBLUEBALL = 4 };
@@ -93,6 +96,15 @@ enum : int { BABYAI_REDBALL_GREY = 0, BABYAI_REDBALL = 1, BABYAI_OBJ = 2, BABYAI
 enum : int { BABYAI_ONEROOM = 0, BABYAI_PICKUPDIST = 1, BABYAI_PUTNEXTLOCAL = 2 };
 // level_aux of a Pickup level: which parts of ObjDesc(type, colour) are set, and PickupInstr's strict flag
 enum : uint32_t { PICK_TYPE = 1u, PICK_COLOR = 2u, PICK_STRICT = 4u };
+// kp[4] of RG_BABYAI_OPEN; kp[5] is OpenDoor's select_by (0 colour, 1 loc, 2 drawn), OpenTwoDoors' fixed red / blue
+// colours (0 or 1), OpenDoorsOrder's num_doors (2..4) or UnlockLocal's distractors (0 or 1); kp[6] strict / debug
+enum : int { BABYAI_OPENREDDOOR = 0, BABYAI_OPENDOOR = 1, BABYAI_OPENTWODOORS = 2, BABYAI_OPENDOORSORDER = 3,
+             BABYAI_UNLOCKLOCAL = 4 };
+// level_aux of an Open level. level_tx / level_ty are the doors the first / second OpenInstr's obj_set holds, as a mask
+// of door colours (every door of these levels has a colour of its own); OPEN_SEQ: two OpenInstrs in sequence (an
+// AfterInstr is stored with its two instructions swapped), OPEN_STRICT1 / 2: their strict flags; OPEN_DONE: the first
+// has succeeded (BeforeInstr.a_done / AfterInstr.b_done), the one bit K1 changes during an episode
+enum : uint32_t { OPEN_SEQ = 1u, OPEN_STRICT1 = 2u, OPEN_STRICT2 = 4u, OPEN_DONE = 8u };
 enum : int { AUTORESET_NEXT_STEP = 0, AUTORESET_SAME_STEP = 1, AUTORESET_DISABLED = 2 };
 // bits of the sticky device error word (Params::err)
 enum : int { ERR_BAD_ACTION = 1, ERR_BAD_STATE = 2, ERR_PACKED_RANGE = 4 };

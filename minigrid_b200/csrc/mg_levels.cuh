@@ -498,7 +498,77 @@ MG_D void draw_level(const Params &p, Pcg &r, Level &L) {
       return !(objs & ~reach);
     };
     int dpx = 0, dpy = 0;
-    if (variant == RG_BABYAI_PICKUP_PUTNEXT) {
+    if (variant == RG_BABYAI_OPEN) {
+      // RoomGridLevel._gen_grid (babyai/core/roomgrid_level.py:119-177) with the gen_mission of OpenRedDoor (open.py:143-146),
+      // OpenDoor (open.py:210-229), OpenTwoDoors (open.py:306-324), OpenDoorsOrder (open.py:399-423) and UnlockLocal
+      // (unlock.py:168-175). None of them rejects a level. Every door is one of room (1, 1)'s (room (0, 0)'s for
+      // OpenRedDoor), and each has a colour of its own, so an OpenInstr's obj_set is a mask of door colours.
+      const int level = p.kp[4], arg = p.kp[5];
+      const uint32_t strict = p.kp[6] ? 1u : 0u;
+      uint32_t m1 = 0, m2 = 0, aux = 0;
+      int c[4], px[4], py[4];
+      auto rand_colors = [&](int n) {  // _rand_subset(COLOR_NAMES, n): _rand_elem on the shrinking sorted list
+        uint32_t left = 0403512u;
+        for (int k = 0; k < n; ++k) {
+          const int pick = rng_integers(r, 0, 6 - k);
+          c[k] = (int)((left >> (3 * pick)) & 7u);
+          left = (left & ((1u << (3 * pick)) - 1u)) | ((left >> (3 * (pick + 1))) << (3 * pick));
+        }
+      };
+      if (level == BABYAI_OPENREDDOOR) {  // OpenInstr(ObjDesc("door", "red"))
+        add_door(0, 0, 0, (int)C_RED, 0, px[0], py[0]);
+        place_agent(0, 0);
+        m1 = 1u << C_RED;
+      } else if (level == BABYAI_OPENDOOR) {
+        rand_colors(4);
+        for (int k = 0; k < 4; ++k) add_door(1, 1, k, c[k], 0, px[k], py[k]);
+        const int select_by = arg == 2 ? rng_integers(r, 0, 2) : arg;  // _rand_elem(["color", "loc"]) when None
+        const int loc = select_by == 1 ? rng_integers(r, 0, 4) : 0;    // _rand_elem(LOC_NAMES): left right front behind
+        place_agent(1, 1);
+        if (select_by == 0) m1 = 1u << c[0];  // ObjDesc("door", color=objs[0].color)
+        else {
+          // find_matching_objs (verifier.py:105-171) at reset: the doors of the agent's room (pos_inside includes the
+          // walls) on the side of the agent that loc names, against its direction d1 and d2 = (-d1.y, d1.x)
+          const int d1x = (L.adir == 0) - (L.adir == 2), d1y = (L.adir == 1) - (L.adir == 3);
+          for (int k = 0; k < 4; ++k) {
+            const int vx = px[k] - L.ax, vy = py[k] - L.ay, v1 = vx * d1x + vy * d1y, v2 = vy * d1x - vx * d1y;
+            if (loc == 0 ? v2 < 0 : loc == 1 ? v2 > 0 : loc == 2 ? v1 > 0 : v1 < 0) m1 |= 1u << c[k];
+          }
+        }
+        aux = strict ? OPEN_STRICT1 : 0u;
+      } else if (level == BABYAI_OPENTWODOORS) {
+        rand_colors(2);  // drawn even when the red / blue ids then ignore them
+        const int first = arg ? (int)C_RED : c[0], second = arg ? (int)C_BLUE : c[1];
+        add_door(1, 1, 2, first, 0, px[0], py[0]);
+        add_door(1, 1, 0, second, 0, px[1], py[1]);
+        place_agent(1, 1);
+        m1 = 1u << first; m2 = 1u << second;  // BeforeInstr(OpenInstr(door1, strict), OpenInstr(door2))
+        aux = OPEN_SEQ | (strict ? OPEN_STRICT1 : 0u);
+      } else if (level == BABYAI_OPENDOORSORDER) {
+        rand_colors(arg);
+        for (int k = 0; k < arg; ++k) add_door(1, 1, -1, c[k], 0, px[k], py[k]);  // the side is drawn until a free one
+        place_agent(1, 1);
+        // door1, door2 = _rand_subset(doors, 2): the second draw indexes the list without the first
+        const int i1 = rng_integers(r, 0, arg), i2r = rng_integers(r, 0, arg - 1), i2 = i2r < i1 ? i2r : i2r + 1;
+        const int mode = rng_integers(r, 0, 3);  // OpenInstr(desc1), BeforeInstr(desc1, desc2), AfterInstr(desc1, desc2)
+        m1 = 1u << c[mode == 2 ? i2 : i1];
+        if (mode != 0) m2 = 1u << c[mode == 2 ? i1 : i2];
+        aux = (mode != 0 ? OPEN_SEQ : 0u) | (strict ? OPEN_STRICT1 | OPEN_STRICT2 : 0u);
+      } else {  // UnlockLocal: a locked door (side, then colour drawn), its key, distractors, OpenInstr(ObjDesc("door"))
+        const int col = add_door(1, 1, -1, -1, 1, px[0], py[0]);
+        add_object(1, 1, 0, col);  // reject_next_to is relative to the default agent position, the middle of room (1, 1)
+        while (arg && L.nrooms < 4) {  // add_distractors(1, 1, 3, all_unique=True): the key counts as existing
+          const uint32_t dc = color_name_idx(rng_integers(r, 0, 6));
+          const uint32_t kind = (uint32_t)rng_integers(r, 0, 3);
+          bool dup = false;
+          for (int k = 0; k < L.nrooms; ++k) dup |= ((rg_obj(L, k) >> 10) & 31u) == (kind | (dc << 2));
+          if (!dup) add_object(1, 1, (int)kind, (int)dc);
+        }
+        place_agent(1, 1);
+        m1 = 0x3Fu;
+      }
+      level_target(L, (int)m1, (int)m2, aux);
+    } else if (variant == RG_BABYAI_PICKUP_PUTNEXT) {
       // RoomGridLevel._gen_grid (babyai/core/roomgrid_level.py:119-177) with the gen_mission of OneRoomS* (other.py:329-332),
       // PickupDist (pickup.py:275-290) and PutNextLocal (putnext.py:71-80), then validate_instrs; RejectSampling starts
       // the next attempt from an empty room while the stream continues. As for GoTo, place_obj's RecursionError is not

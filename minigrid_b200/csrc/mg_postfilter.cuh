@@ -29,7 +29,8 @@ struct PostIn {
   // roomgrid only: kp[0], and whether the cell at (tx, ty) is an open door after the transition (Unlock's self.door.is_open)
   int variant;
   bool door_open;
-  // roomgrid BabyAI GoTo only: the code of the cell in front of the agent after the transition (0 = not read)
+  // roomgrid BabyAI GoTo, and BabyAI Open on a toggle: the code of the cell in front of the agent after the transition
+  // (0 = not read)
   uint32_t front = 0;
   // roomgrid BabyAI Pickup / PutNext only: kp[4], and on a drop the codes of the three cells next to the front cell other
   // than the agent's, one per byte, after the transition (0 = not read)
@@ -37,11 +38,24 @@ struct PostIn {
   uint32_t next_to = 0;
 };
 enum : int { POST_KEEP = 0, POST_REWARD = 1, POST_ZERO = 2 };  // what becomes of the step's reward
-struct PostOut { uint32_t terminated; int reward; };
+// aux: level_aux after the step; only the BabyAI Open levels change it (OPEN_DONE), K1 stores it back with the record
+struct PostOut { uint32_t terminated; int reward; uint32_t aux = 0; };
+
+// OpenInstr.verify_action (babyai/core/verifier.py:270-287) of one instruction whose obj_set is the door colour mask
+// `doors`, on a toggle: success when the front cell is now an open door of obj_set (doors never move or change colour,
+// so "front_cell is door" is "the front cell is a door whose colour is in the mask"); otherwise, when strict and the
+// front cell is a door in any state, failure
+enum : int { OPEN_CONTINUE = 0, OPEN_SUCCESS = 1, OPEN_FAILURE = 2 };
+MG_HD int open_verify(uint32_t front, int doors, bool strict) {
+  const uint32_t t4 = front & 15u;
+  const bool door = t4 == T_DOOR || t4 == T4_DOOR_CLOSED || t4 == T4_DOOR_LOCKED;
+  if (t4 == T_DOOR && ((doors >> ((front >> 4) & 7u)) & 1)) return OPEN_SUCCESS;
+  return (strict && door) ? OPEN_FAILURE : OPEN_CONTINUE;
+}
 
 template <int KIND>
 MG_HD PostOut post_filter(const PostIn &in, uint32_t terminated) {
-  PostOut o = {terminated, POST_KEEP};
+  PostOut o = {terminated, POST_KEEP, in.aux};
   if (KIND == KIND_GOTODOOR || KIND == KIND_GOTOOBJECT) {  // gotodoor.py:130-149, gotoobject.py:141-160
     if (in.action == A_TOGGLE) o.terminated = 1u;
     if (in.action == A_DONE) {
@@ -96,6 +110,25 @@ MG_HD PostOut post_filter(const PostIn &in, uint32_t terminated) {
                            (!(in.aux & PICK_COLOR) || (int)((in.carry >> 4) & 7u) == in.ty);
         if (in.carry_before == 0u && match) { o.reward = POST_REWARD; o.terminated = 1u; }
         else if ((in.aux & PICK_STRICT) && in.carry != 0u) { o.reward = POST_ZERO; o.terminated = 1u; }
+      }
+    } else if (in.variant == RG_BABYAI_OPEN) {
+      // RoomGridLevel.step (babyai/core/roomgrid_level.py:87-104). OpenInstr answers "continue" to every action but
+      // toggle, and so does a sequence of two. BeforeInstr.verify / AfterInstr.verify (verifier.py:467-530, strict=False)
+      // verify the first instruction until it succeeds, then verify the second ON THE SAME ACTION: a strict second
+      // OpenInstr sees the first one's door, which is not its own, and fails the episode.
+      if (in.action == A_TOGGLE) {
+        int st;
+        if (!(in.aux & OPEN_DONE)) {
+          st = open_verify(in.front, in.tx, (in.aux & OPEN_STRICT1) != 0u);
+          if (st == OPEN_SUCCESS && (in.aux & OPEN_SEQ)) {
+            o.aux = in.aux | OPEN_DONE;
+            st = open_verify(in.front, in.ty, (in.aux & OPEN_STRICT2) != 0u);
+          }
+        } else {
+          st = open_verify(in.front, in.ty, (in.aux & OPEN_STRICT2) != 0u);
+        }
+        if (st == OPEN_SUCCESS) { o.reward = POST_REWARD; o.terminated = 1u; }
+        if (st == OPEN_FAILURE) { o.reward = POST_ZERO; o.terminated = 1u; }
       }
     } else if (in.variant == RG_UNLOCK) {  // unlock.py:88-96
       if (in.action == A_TOGGLE && in.door_open) { o.reward = POST_REWARD; o.terminated = 1u; }

@@ -578,7 +578,8 @@ k_step(const __grid_constant__ Params p, const void *__restrict__ actions, int a
         in.tx = tx; in.ty = ty; in.aux = flags >> 8;
         in.red_before = in.blue_before = in.red_after = in.blue_after = false;
         in.variant = p.kp[0]; in.door_open = false; in.front = 0;
-        if (KIND == KIND_ROOMGRID && p.kp[0] == RG_BABYAI_GOTO) {  // the front cell after this step's turn, move or mutation
+        // the front cell after this step's turn, move or mutation (GoTo on every step, Open on a toggle)
+        if (KIND == KIND_ROOMGRID && (p.kp[0] == RG_BABYAI_GOTO || (p.kp[0] == RG_BABYAI_OPEN && act == A_TOGGLE))) {
           if (WIN) {  // the loaded words hold the agent's line for its new direction, the mutation included
             in.front = view_words_byte(vw, ((dir & 1) ? ay : ax) + ((dir < 2) ? 1 : -1));
           } else {
@@ -612,6 +613,7 @@ k_step(const __grid_constant__ Params p, const void *__restrict__ actions, int a
         }
         const PostOut po = post_filter<KIND>(in, terminated);
         terminated = po.terminated;
+        if (KIND == KIND_ROOMGRID) flags = (flags & 0xFFu) | (po.aux << 8);  // BabyAI Open's progress bit
         if (po.reward == POST_ZERO) reward = 0.0;
         if (po.reward == POST_REWARD)
           reward = steps <= p.max_steps ? p.reward_lut[steps]

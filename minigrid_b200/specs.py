@@ -286,13 +286,56 @@ BABYAI_PICKUP_PUTNEXT_REGISTRY = {
 }
 
 
+BABYAI_OPEN = 9  # roomgrid variant of the BabyAI Open and UnlockLocal levels
+BABYAI_OPENREDDOOR, BABYAI_OPENDOOR, BABYAI_OPENTWODOORS, BABYAI_OPENDOORSORDER, BABYAI_UNLOCKLOCAL = 0, 1, 2, 3, 4
+_SELECT_BY = {"color": 0, "loc": 1, None: 2}
+
+
+def babyai_open(level, mission, room_size=8, num_rows=3, num_cols=3, arg=0, strict=False, max_steps=None):
+    """envs/babyai/open.py and unlock.py (UnlockLocal): max_steps = room_size^2 * num_rows * num_cols for one navigation
+    (roomgrid_level.py:71-85), or the fixed 20 * 6^2 of OpenTwoDoors and OpenDoorsOrder. `arg` is OpenDoor's select_by,
+    OpenTwoDoors' fixed red / blue colours, OpenDoorsOrder's num_doors or UnlockLocal's distractors."""
+    steps = max_steps or room_size * room_size * num_rows * num_cols
+    return roomgrid(BABYAI_OPEN, room_size, num_rows, num_cols, steps, mission, (level, int(arg), int(strict)))
+
+
+# OpenDoor's descriptor is a colour ("open the red door") or a location against the agent's pose at reset ("open a door
+# on your left", "open the door in front of you"); OpenDoorsOrder's instruction is one OpenInstr, or two joined by
+# ", then " (BeforeInstr) or " after you " (AfterInstr)
+_OPEN_DOOR = "open {article} {color} door {location}"
+_OPEN_ORDER = "open the {color} door[, then open the {color} door| after you open the {color} door]"
+
+# __init__.py:774-844, 957-965 (the BabyAI Open levels without connect_all, and UnlockLocal)
+BABYAI_OPEN_REGISTRY = {
+    "BabyAI-OpenRedDoor-v0": babyai_open(BABYAI_OPENREDDOOR, "open the red door", 5, 1, 2),
+    "BabyAI-OpenDoor-v0": babyai_open(BABYAI_OPENDOOR, _OPEN_DOOR, arg=_SELECT_BY[None]),
+    "BabyAI-OpenDoorDebug-v0": babyai_open(BABYAI_OPENDOOR, _OPEN_DOOR, arg=_SELECT_BY[None], strict=True),
+    "BabyAI-OpenDoorColor-v0": babyai_open(BABYAI_OPENDOOR, "open the {color} door", arg=_SELECT_BY["color"]),
+    "BabyAI-OpenDoorLoc-v0": babyai_open(BABYAI_OPENDOOR, "open {article} door {location}", arg=_SELECT_BY["loc"]),
+    "BabyAI-OpenTwoDoors-v0": babyai_open(BABYAI_OPENTWODOORS, "open the {color} door, then open the {color} door", 6,
+                                          max_steps=720),
+    "BabyAI-OpenRedBlueDoors-v0": babyai_open(BABYAI_OPENTWODOORS, "open the red door, then open the blue door", 6,
+                                              arg=1, max_steps=720),
+    "BabyAI-OpenRedBlueDoorsDebug-v0": babyai_open(BABYAI_OPENTWODOORS, "open the red door, then open the blue door", 6,
+                                                   arg=1, strict=True, max_steps=720),
+    **{f"BabyAI-OpenDoorsOrderN{n}{dbg}-v0": babyai_open(BABYAI_OPENDOORSORDER, _OPEN_ORDER, 6, arg=n, strict=bool(dbg),
+                                                          max_steps=720)
+       for dbg in ("", "Debug") for n in (2, 4)},
+    "BabyAI-UnlockLocal-v0": babyai_open(BABYAI_UNLOCKLOCAL, "open the door"),
+    "BabyAI-UnlockLocalDist-v0": babyai_open(BABYAI_UNLOCKLOCAL, "open the door", arg=1),
+}
+
+
 def get(env_id: str) -> EnvSpec:
     if env_id in BABYAI_REGISTRY:
         return BABYAI_REGISTRY[env_id]
     if env_id in BABYAI_PICKUP_PUTNEXT_REGISTRY:
         return BABYAI_PICKUP_PUTNEXT_REGISTRY[env_id]
+    if env_id in BABYAI_OPEN_REGISTRY:
+        return BABYAI_OPEN_REGISTRY[env_id]
     try:
         return REGISTRY[env_id]
     except KeyError:
         raise KeyError(f"{env_id!r} is not one of the ids this engine implements: "
-                       f"{sorted(REGISTRY) + sorted(BABYAI_REGISTRY) + sorted(BABYAI_PICKUP_PUTNEXT_REGISTRY)}") from None
+                       f"{sorted(REGISTRY) + sorted(BABYAI_REGISTRY) + sorted(BABYAI_PICKUP_PUTNEXT_REGISTRY) + sorted(BABYAI_OPEN_REGISTRY)}"
+                       ) from None

@@ -1,4 +1,4 @@
-"""BabyAI GoTo env-steps/s on the GPU, and the cost of the BabyAI branch to the existing roomgrid kinds.
+"""BabyAI env-steps/s on the GPU, and the cost of the BabyAI branch to the existing roomgrid kinds.
 
     python scripts/bench_babyai.py [--ids ID,...] [--parent DIR] [--ab-ids ID,...] [--repeats 3] [--steps 400]
 
@@ -18,7 +18,8 @@ import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-IDS = ["BabyAI-GoToLocal-v0", "BabyAI-GoToRedBallGrey-v0", "BabyAI-GoToRedBlueBall-v0"]
+IDS = ["BabyAI-GoToLocal-v0", "BabyAI-GoToRedBallGrey-v0", "BabyAI-GoToRedBlueBall-v0", "BabyAI-OpenRedDoor-v0",
+       "BabyAI-OpenDoor-v0", "BabyAI-OpenDoorsOrderN4-v0", "BabyAI-UnlockLocalDist-v0"]
 AB_IDS = ["MiniGrid-DoorKey-8x8-v0", "MiniGrid-KeyCorridorS6R3-v0"]
 
 
