@@ -211,6 +211,26 @@ int mg_obs_rgb_partial(mg_env *env, const uint8_t *image_dev, const uint8_t *til
 int mg_obs_rgb_full(mg_env *env, const uint8_t *image_dev, const uint8_t *tiles_dev, const uint16_t *index_dev,
                     uint8_t *out_dev, void *stream);
 
+/* Per-episode missions of the BabyAI levels (roomgrid variants 7..9).
+ *  mg_enable_missions    the handle keeps one mission code per env (uint32, layout in mg_common.cuh: MIS_*), written by
+ *                        every reset and autoreset: RoomGridLevel._gen_grid's self.mission = self.instrs.surface(self)
+ *                        (babyai/core/roomgrid_level.py:142-144) in encoded form. Only before the handle's first mg_seed*,
+ *                        mg_reset* or step; refused for the MiniGrid kinds that draw their mission (LockedRoom, GoToDoor,
+ *                        Fetch, GoToObject, PutNear, UnlockPickup, BlockedUnlockPickup, KeyCorridor). For the other
+ *                        non-BabyAI ids it is a no-op: their codes stay 0, "the spec's constant string".
+ *  mg_get_mission_codes  out_dev uint32[n]: the codes (MiniGridEnv.mission of every env, before rendering)
+ *  mg_mission_text       out_dev uint8[n][96] (16-byte aligned): MiniGridEnv.mission, zero padded (empty for code 0)
+ *  mg_mission_indices    out_dev int64[n][max_words]: DictObservationSpaceWrapper.observation (wrappers.py:535-554), word
+ *                        index + 1 in get_minigrid_words(), zero padded; -1 for a word outside that vocabulary
+ *  mg_obs_flat_missions  FlatObsWrapper.observation (wrappers.py:589-626) with each env's own mission: out_dev
+ *                        uint8[n][image_bytes + 28 * 96]
+ * The three render calls need a BabyAI level with missions enabled. mg_set_state leaves the codes as they are. */
+int mg_enable_missions(mg_env *env);
+int mg_get_mission_codes(mg_env *env, uint32_t *out_dev, void *stream);
+int mg_mission_text(mg_env *env, uint8_t *out_dev, void *stream);
+int mg_mission_indices(mg_env *env, int max_words, int64_t *out_dev, void *stream);
+int mg_obs_flat_missions(mg_env *env, const uint8_t *image_dev, int image_bytes, uint8_t *out_dev, void *stream);
+
 /* Replaces: pickling / inspecting env objects (tests/test_envs.py:185-195) and lets tests inject states.
  * grid_dev: Grid.encode() uint8[n][W][H][3]; agent_dev: int32[n][6] {x, y, dir, carry_type (-1 none),
  * carry_color, step_count}; rng_dev: uint64[n][6] {state_hi, state_lo, inc_hi, inc_lo, has_uint32,

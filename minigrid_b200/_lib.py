@@ -17,6 +17,7 @@ EXPORTS = [
     "mg_reset", "mg_seed_masked", "mg_reset_masked", "mg_step", "mg_gen_obs", "mg_reset_host", "mg_step_host", "mg_full_obs", "mg_get_state", "mg_set_state",
     "mg_check_error", "mg_profile", "mg_profile_read", "mg_set_host_format", "mg_host_d2h_bytes", "mg_host_threads", "mg_expand_packed", "mg_expand_packed_mt", "mg_obs_view", "mg_obs_onehot", "mg_obs_flat", "mg_obs_symbolic",
     "mg_obs_rgb_partial", "mg_obs_rgb_full", "mg_hash",
+    "mg_enable_missions", "mg_get_mission_codes", "mg_mission_text", "mg_mission_indices", "mg_obs_flat_missions",
 ]
 
 
@@ -73,6 +74,11 @@ def load(build_if_missing: bool = True):
     L.mg_obs_rgb_full.argtypes = [p, p, p, p, p, p]
     L.mg_expand_packed.argtypes = [p, i64, i32, p, p, p, p, p]
     L.mg_expand_packed_mt.argtypes = [p, i64, i32, p, p, p, p, p, i32]
+    L.mg_enable_missions.argtypes = [p]
+    L.mg_get_mission_codes.argtypes = [p, p, p]
+    L.mg_mission_text.argtypes = [p, p, p]
+    L.mg_mission_indices.argtypes = [p, i32, p, p]
+    L.mg_obs_flat_missions.argtypes = [p, p, i32, p, p]
     L.mg_get_state.argtypes = [p] * 6
     L.mg_set_state.argtypes = [p] * 6
     L.mg_check_error.argtypes = [p, p]

@@ -37,6 +37,9 @@ cudaError_t launch_symbolic(const Params &p, long long *out, cudaStream_t s);
 cudaError_t launch_rgb_partial(const uint8_t *img, const uint8_t *tiles, const uint16_t *index, uint8_t *out, long long n_envs, cudaStream_t s);
 cudaError_t launch_rgb_full(const Params &p, const uint8_t *img, const uint8_t *tiles, const uint16_t *index, uint8_t *out, cudaStream_t s);
 cudaError_t launch_template(const Params &p, uint32_t *tmpl, cudaStream_t stream);
+cudaError_t launch_mission_text(const uint32_t *codes, uint8_t *out, int n, cudaStream_t s);
+cudaError_t launch_mission_indices(const uint32_t *codes, long long *out, int max_words, int n, cudaStream_t s);
+cudaError_t launch_flat_missions(const uint8_t *img, int img_bytes, const uint32_t *codes, uint8_t *out, int n, cudaStream_t s);
 cudaError_t configure_hash(const Params &p, int *grid);
 cudaError_t launch_hash(const Params &p, int grid, const uint4 *tmpl, int form0, uint8_t *digest, cudaStream_t stream);
 }  // namespace mg
@@ -82,6 +85,9 @@ struct mg_env {
   // MiniGridEnv.hash (mg_hash.cu): the prefix template of this geometry, the kind's form of agent_pos after a reset
   const uint4 *d_hash_tmpl;
   int hash_form, hash_grid;
+  // mg_enable_missions: allowed while no seed, reset or step has touched the envs; the roomgrid kind then keeps the
+  // codes in p.extra (mission_codes()), the other kinds' missions are constant (code 0)
+  int touched, missions;
 };
 
 static thread_local std::string g_err;
@@ -366,6 +372,7 @@ int mg_destroy(mg_env *h) {
   cudaFree(h->d_packed);
   cudaFreeHost(h->h_packed);
   cudaFree(h->p.counts);
+  if (h->p.kind == KIND_ROOMGRID) cudaFree(h->p.extra);  // the mission codes (KIND_DYNOBS: `extra` lies in the arena)
   free(h->h_reward_lut);
   for (int c = 0; c < 16; ++c)
     if (h->chunk_ev[c]) cudaEventDestroy(h->chunk_ev[c]);
@@ -426,6 +433,7 @@ static int seed_impl(mg_env *h, const uint8_t *mask_dev, const uint64_t *seeds_h
   MG_ON_DEVICE(h);
   cudaStream_t s = (cudaStream_t)stream;
   note_stream(h, s);
+  h->touched = 1;
   if (seeds_host) {
     if (!h->d_seeds) MG_CUDA(cudaMalloc(&h->d_seeds, (size_t)h->p.n_envs * sizeof(uint64_t)));
     MG_CUDA(cudaMemcpyAsync(h->d_seeds, seeds_host, (size_t)h->p.n_envs * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
@@ -458,6 +466,7 @@ int mg_reset(mg_env *h, uint8_t *obs_dev, int32_t *dir_dev, void *stream) {
   MG_ON_DEVICE(h);
   cudaStream_t s = (cudaStream_t)stream;
   note_stream(h, s);
+  h->touched = 1;
   MG_CUDA(launch_reset(h->p, nullptr, obs_dev, dir_dev, s));
   h->launches += 1;
   return MG_OK;
@@ -468,6 +477,7 @@ int mg_reset_masked(mg_env *h, const uint8_t *mask_dev, uint8_t *obs_dev, int32_
   MG_ON_DEVICE(h);
   cudaStream_t s = (cudaStream_t)stream;
   note_stream(h, s);
+  h->touched = 1;
   MG_CUDA(launch_reset(h->p, mask_dev, obs_dev, dir_dev, s));
   h->launches += 1;
   return MG_OK;
@@ -480,6 +490,7 @@ int mg_step(mg_env *h, const void *actions_dev, int action_dtype, uint8_t *obs_d
   MG_ON_DEVICE(h);
   cudaStream_t s = (cudaStream_t)stream;
   note_stream(h, s);
+  h->touched = 1;
   const Params &p = h->p;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   if (h->profiling) {
@@ -600,6 +611,74 @@ int mg_obs_rgb_full(mg_env *h, const uint8_t *image_dev, const uint8_t *tiles_de
   MG_ON_DEVICE(h);
   note_stream(h, (cudaStream_t)stream);
   MG_CUDA(launch_rgb_full(h->p, image_dev, tiles_dev, index_dev, out_dev, (cudaStream_t)stream));
+  h->launches += 1;
+  return MG_OK;
+}
+
+// ---- per-episode missions of the BabyAI levels (mg_mission.cu) ----
+int mg_enable_missions(mg_env *h) {
+  if (!h) return fail(MG_ERR_INVALID_ARG, "mg_enable_missions: NULL handle");
+  if (h->missions) return MG_OK;
+  if (h->touched) return fail(MG_ERR_INVALID_ARG, "mg_enable_missions: only before the handle's first seed, reset or step");
+  const int k = h->p.kind, variant = h->p.kp[0];
+  if (k == KIND_LOCKEDROOM || k == KIND_GOTODOOR || k == KIND_FETCH || k == KIND_GOTOOBJECT || k == KIND_PUTNEAR ||
+      (k == KIND_ROOMGRID && (variant == RG_UNLOCKPICKUP || variant == RG_BLOCKEDUNLOCKPICKUP || variant == RG_KEYCORRIDOR)))
+    return fail(MG_ERR_INVALID_ARG, "mg_enable_missions: missions drawn per episode are produced for the BabyAI levels only; "
+                                    "this MiniGrid level's mission names what it drew and is not encoded");
+  if (k != KIND_ROOMGRID) { h->missions = 1; return MG_OK; }  // a constant mission string: every code stays MIS_CONST
+  MG_ON_DEVICE(h);
+  const size_t bytes = (size_t)h->p.n_tiles * TILE * sizeof(uint32_t);
+  uint32_t *m = nullptr;
+  MG_CUDA(cudaMalloc(&m, bytes));
+  cudaError_t e = cudaMemset(m, 0, bytes);
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  if (e != cudaSuccess) { cudaFree(m); return fail(MG_ERR_CUDA, std::string("mg_enable_missions: ") + cudaGetErrorString(e)); }
+  h->p.extra = reinterpret_cast<uint4 *>(m);
+  h->missions = 1;
+  return MG_OK;
+}
+// the render calls: the codes of a BabyAI level
+static int need_missions(mg_env *h, const char *fn) {
+  if (!h->missions) return fail(MG_ERR_INVALID_ARG, std::string(fn) + ": the handle has no missions (mg_enable_missions)");
+  if (h->p.kind != KIND_ROOMGRID || h->p.kp[0] < RG_BABYAI_GOTO)
+    return fail(MG_ERR_INVALID_ARG, std::string(fn) + ": only the BabyAI levels' missions are encoded per env");
+  return MG_OK;
+}
+int mg_get_mission_codes(mg_env *h, uint32_t *out_dev, void *stream) {
+  if (!h || !out_dev) return fail(MG_ERR_INVALID_ARG, "mg_get_mission_codes: NULL argument");
+  if (!h->missions) return fail(MG_ERR_INVALID_ARG, "mg_get_mission_codes: the handle has no missions (mg_enable_missions)");
+  MG_ON_DEVICE(h);
+  note_stream(h, (cudaStream_t)stream);
+  const size_t bytes = (size_t)h->p.n_envs * sizeof(uint32_t);
+  if (h->p.kind == KIND_ROOMGRID) MG_CUDA(cudaMemcpyAsync(out_dev, mission_codes(h->p), bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  else MG_CUDA(cudaMemsetAsync(out_dev, 0, bytes, (cudaStream_t)stream));
+  return MG_OK;
+}
+int mg_mission_text(mg_env *h, uint8_t *out_dev, void *stream) {
+  if (!h || !out_dev) return fail(MG_ERR_INVALID_ARG, "mg_mission_text: NULL argument");
+  if ((uintptr_t)out_dev & 15u) return fail(MG_ERR_INVALID_ARG, "mg_mission_text: out_dev must be 16-byte aligned");
+  if (int rc = need_missions(h, "mg_mission_text")) return rc;
+  MG_ON_DEVICE(h);
+  note_stream(h, (cudaStream_t)stream);
+  MG_CUDA(launch_mission_text(mission_codes(h->p), out_dev, h->p.n_envs, (cudaStream_t)stream));
+  h->launches += 1;
+  return MG_OK;
+}
+int mg_mission_indices(mg_env *h, int max_words, int64_t *out_dev, void *stream) {
+  if (!h || !out_dev || max_words < 1) return fail(MG_ERR_INVALID_ARG, "mg_mission_indices: bad argument");
+  if (int rc = need_missions(h, "mg_mission_indices")) return rc;
+  MG_ON_DEVICE(h);
+  note_stream(h, (cudaStream_t)stream);
+  MG_CUDA(launch_mission_indices(mission_codes(h->p), (long long *)out_dev, max_words, h->p.n_envs, (cudaStream_t)stream));
+  h->launches += 1;
+  return MG_OK;
+}
+int mg_obs_flat_missions(mg_env *h, const uint8_t *image_dev, int image_bytes, uint8_t *out_dev, void *stream) {
+  if (!h || !image_dev || !out_dev || image_bytes < 1) return fail(MG_ERR_INVALID_ARG, "mg_obs_flat_missions: bad argument");
+  if (int rc = need_missions(h, "mg_obs_flat_missions")) return rc;
+  MG_ON_DEVICE(h);
+  note_stream(h, (cudaStream_t)stream);
+  MG_CUDA(launch_flat_missions(image_dev, image_bytes, mission_codes(h->p), out_dev, h->p.n_envs, (cudaStream_t)stream));
   h->launches += 1;
   return MG_OK;
 }
@@ -861,6 +940,7 @@ int mg_step_host(mg_env *h, const int32_t *actions_host, uint8_t *obs_host, int3
     src = h->h_actions;
   }
   order_after_caller(h);
+  h->touched = 1;
   if (h->host_format == MG_HOST_PACKED)
     return step_host_packed(h, src, obs_host, dir_host, reward_host, terminated_host, truncated_host);
   MG_CUDA(cudaMemcpyAsync(h->d_actions, src, n * sizeof(int32_t), cudaMemcpyHostToDevice, h->hstream));

@@ -105,6 +105,27 @@ enum : int { BABYAI_OPENREDDOOR = 0, BABYAI_OPENDOOR = 1, BABYAI_OPENTWODOORS = 
 // AfterInstr is stored with its two instructions swapped), OPEN_STRICT1 / 2: their strict flags; OPEN_DONE: the first
 // has succeeded (BeforeInstr.a_done / AfterInstr.b_done), the one bit K1 changes during an episode
 enum : uint32_t { OPEN_SEQ = 1u, OPEN_STRICT1 = 2u, OPEN_STRICT2 = 4u, OPEN_DONE = 8u };
+// Mission code of a BabyAI level (Params::mission, one word per env, written by every reset when the handle asked for
+// missions): the instruction that RoomGridLevel._gen_grid turns into self.mission = self.instrs.surface(self)
+// (babyai/core/roomgrid_level.py:142-144), rendered back into text by mission_words (mg_mission.cuh).
+//   bits  0-2   form: MIS_CONST the spec's constant string (every id that is not a BabyAI level), MIS_GOTO "go to A",
+//               MIS_PICKUP "pick up A", MIS_OPEN "open A", MIS_PUTNEXT "put A next to B", MIS_BEFORE "open A, then open B"
+//               (BeforeInstr), MIS_AFTER "open A after you open B" (AfterInstr, in the reference's surface order:
+//               instr_a first, although level_tx / level_ty hold it swapped)
+//   bits  3-12  ObjDesc A, bits 13-22 ObjDesc B, 10 bits each (verifier.py:44-100):
+//               type:3   0 none ("object"), 1 key, 2 ball, 3 box, 4 door
+//               colour:3 0 none, 1 + COLOR_TO_IDX
+//               loc:3    0 none, 1 left, 2 right, 3 front, 4 behind (LOC_NAMES order)
+//               plural:1 len(obj_set) > 1 at reset: "a" instead of "the"
+//   bits 23-31  zero (forms 7 and up and these bits are free for missions of other levels)
+enum : uint32_t { MIS_CONST = 0, MIS_GOTO = 1, MIS_PICKUP = 2, MIS_OPEN = 3, MIS_PUTNEXT = 4, MIS_BEFORE = 5, MIS_AFTER = 6 };
+enum : uint32_t { MIS_TYPE_NONE = 0, MIS_TYPE_KEY = 1, MIS_TYPE_BALL = 2, MIS_TYPE_BOX = 3, MIS_TYPE_DOOR = 4 };
+enum : uint32_t { MIS_LOC_NONE = 0, MIS_LOC_LEFT = 1, MIS_LOC_RIGHT = 2, MIS_LOC_FRONT = 3, MIS_LOC_BEHIND = 4 };
+// one ObjDesc: type MIS_TYPE_*, colour COLOR_TO_IDX or -1 for none, loc MIS_LOC_*
+MG_HD uint32_t mission_desc(uint32_t type, int color, uint32_t loc, bool plural) {
+  return type | ((color < 0 ? 0u : (uint32_t)color + 1u) << 3) | (loc << 6) | ((plural ? 1u : 0u) << 9);
+}
+MG_HD uint32_t mission_code(uint32_t form, uint32_t a, uint32_t b) { return form | (a << 3) | (b << 13); }
 enum : int { AUTORESET_NEXT_STEP = 0, AUTORESET_SAME_STEP = 1, AUTORESET_DISABLED = 2 };
 // bits of the sticky device error word (Params::err)
 enum : int { ERR_BAD_ACTION = 1, ERR_BAD_STATE = 2, ERR_PACKED_RANGE = 4 };
@@ -182,7 +203,10 @@ struct Params {
   int kp[8];                // generator parameters (see include/minigrid_b200.h)
   uint32_t *grid;           // n_tiles * 32 * wpe words, see grid_word()
   uint4 *agent;             // [n_tiles * 32]
-  uint4 *extra;             // [n_tiles * 32], KIND_DYNOBS only: the obstacles in list order, 16 bits each (x | y << 8)
+  // [n_tiles * 32] KIND_DYNOBS: the obstacles in list order, 16 bits each (x | y << 8); KIND_ROOMGRID: the mission codes
+  // (mission_codes()), null unless mg_enable_missions. One slot for both: Params is every kernel's by-value argument,
+  // and a field of its own would move the parameters of every kernel
+  uint4 *extra;
   RngRec *rng;              // [n_tiles * 32]
   const double *reward_lut; // [max_steps + 1], 1 - 0.9 * (k / max_steps) computed on the host in IEEE double
   const uint32_t *cell_lut; // [256] decode_cell()
@@ -198,6 +222,9 @@ struct Params {
   double death_cost;        // NoDeath.death_cost
   uint32_t *counts;         // [n_envs][W * H * 28] (ActionBonus) or [n_envs][W * H] (PositionBonus): the wrappers' self.counts
 };
+
+// KIND_ROOMGRID: one mission code (MIS_*) per env, written by every reset; null unless the handle asked for missions
+MG_HD uint32_t *mission_codes(const Params &p) { return reinterpret_cast<uint32_t *>(p.extra); }
 
 struct StepPlan {  // launch shape of K1, chosen once per handle (mg_step.cu: configure_step)
   int warps, vis, nbuf, mode, ctas_per_sm, grid;

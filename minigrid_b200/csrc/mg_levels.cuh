@@ -40,6 +40,10 @@ MG_D void level_target(Level &L, int tx, int ty, uint32_t aux) {
 MG_D int level_tx(const Level &L) { return (int)(L.ov & 0xFFull); }
 MG_D int level_ty(const Level &L) { return (int)((L.ov >> 8) & 0xFFull); }
 MG_D uint32_t level_aux(const Level &L) { return (uint32_t)((L.ov >> 16) & 0xFFFFull); }
+// KIND_ROOMGRID: the BabyAI generators leave their mission code (MIS_*, mg_common.cuh) in `rv`, which no roomgrid cell
+// function reads; 0 (MIS_CONST) for the other roomgrid variants
+MG_D void level_set_mission(Level &L, uint32_t code) { L.rv = code; }
+MG_D uint32_t level_mission(const Level &L) { return L.rv; }
 
 MG_D uint32_t room_get(const Level &L, int i) {
   return i < 4 ? (uint32_t)(L.rm03 >> (32 * i)) : (uint32_t)(L.rm45 >> (32 * (i - 4)));
@@ -497,6 +501,21 @@ MG_D void draw_level(const Params &p, Pcg &r, Level &L) {
       }
       return !(objs & ~reach);
     };
+    // ObjDesc.find_matching_objs at reset (verifier.py:105-171) in the BabyAI levels' one room: the cells that hold an
+    // object of that kind (0 key, 1 ball, 2 box; -1 any) and colour (-1 any). Every border cell is a grey wall, which a
+    // colour-only grey descriptor matches too.
+    auto n_matching = [&](int kind, int color) -> int {
+      int n = (kind < 0 && color == (int)C_GREY) ? 2 * (W + H) - 4 : 0;
+      for (int k = 0; k < L.nrooms; ++k) {
+        const uint32_t o = rg_obj(L, k);
+        n += (kind < 0 || (int)((o >> 10) & 3u) == kind) && (color < 0 || (int)((o >> 12) & 7u) == color);
+      }
+      return n;
+    };
+    // ObjDesc(kind, colour) of the mission code, "a" when several cells match it
+    auto obj_desc = [&](int kind, int color) -> uint32_t {
+      return mission_desc(kind < 0 ? MIS_TYPE_NONE : MIS_TYPE_KEY + (uint32_t)kind, color, MIS_LOC_NONE, n_matching(kind, color) > 1);
+    };
     int dpx = 0, dpy = 0;
     if (variant == RG_BABYAI_OPEN) {
       // RoomGridLevel._gen_grid (babyai/core/roomgrid_level.py:119-177) with the gen_mission of OpenRedDoor (open.py:143-146),
@@ -505,7 +524,7 @@ MG_D void draw_level(const Params &p, Pcg &r, Level &L) {
       // OpenRedDoor), and each has a colour of its own, so an OpenInstr's obj_set is a mask of door colours.
       const int level = p.kp[4], arg = p.kp[5];
       const uint32_t strict = p.kp[6] ? 1u : 0u;
-      uint32_t m1 = 0, m2 = 0, aux = 0;
+      uint32_t m1 = 0, m2 = 0, aux = 0, mis = 0;
       int c[4], px[4], py[4];
       auto rand_colors = [&](int n) {  // _rand_subset(COLOR_NAMES, n): _rand_elem on the shrinking sorted list
         uint32_t left = 0403512u;
@@ -519,14 +538,17 @@ MG_D void draw_level(const Params &p, Pcg &r, Level &L) {
         add_door(0, 0, 0, (int)C_RED, 0, px[0], py[0]);
         place_agent(0, 0);
         m1 = 1u << C_RED;
+        mis = mission_code(MIS_OPEN, mission_desc(MIS_TYPE_DOOR, (int)C_RED, MIS_LOC_NONE, false), 0u);
       } else if (level == BABYAI_OPENDOOR) {
         rand_colors(4);
         for (int k = 0; k < 4; ++k) add_door(1, 1, k, c[k], 0, px[k], py[k]);
         const int select_by = arg == 2 ? rng_integers(r, 0, 2) : arg;  // _rand_elem(["color", "loc"]) when None
         const int loc = select_by == 1 ? rng_integers(r, 0, 4) : 0;    // _rand_elem(LOC_NAMES): left right front behind
         place_agent(1, 1);
-        if (select_by == 0) m1 = 1u << c[0];  // ObjDesc("door", color=objs[0].color)
-        else {
+        if (select_by == 0) {  // ObjDesc("door", color=objs[0].color)
+          m1 = 1u << c[0];
+          mis = mission_code(MIS_OPEN, mission_desc(MIS_TYPE_DOOR, c[0], MIS_LOC_NONE, false), 0u);
+        } else {
           // find_matching_objs (verifier.py:105-171) at reset: the doors of the agent's room (pos_inside includes the
           // walls) on the side of the agent that loc names, against its direction d1 and d2 = (-d1.y, d1.x)
           const int d1x = (L.adir == 0) - (L.adir == 2), d1y = (L.adir == 1) - (L.adir == 3);
@@ -534,6 +556,8 @@ MG_D void draw_level(const Params &p, Pcg &r, Level &L) {
             const int vx = px[k] - L.ax, vy = py[k] - L.ay, v1 = vx * d1x + vy * d1y, v2 = vy * d1x - vx * d1y;
             if (loc == 0 ? v2 < 0 : loc == 1 ? v2 > 0 : loc == 2 ? v1 > 0 : v1 < 0) m1 |= 1u << c[k];
           }
+          // the colour mask has lost the loc word, so it is kept here; "a door" when several doors lie on that side
+          mis = mission_code(MIS_OPEN, mission_desc(MIS_TYPE_DOOR, -1, MIS_LOC_LEFT + (uint32_t)loc, __popc(m1) > 1), 0u);
         }
         aux = strict ? OPEN_STRICT1 : 0u;
       } else if (level == BABYAI_OPENTWODOORS) {
@@ -543,6 +567,8 @@ MG_D void draw_level(const Params &p, Pcg &r, Level &L) {
         add_door(1, 1, 0, second, 0, px[1], py[1]);
         place_agent(1, 1);
         m1 = 1u << first; m2 = 1u << second;  // BeforeInstr(OpenInstr(door1, strict), OpenInstr(door2))
+        mis = mission_code(MIS_BEFORE, mission_desc(MIS_TYPE_DOOR, first, MIS_LOC_NONE, false),
+                           mission_desc(MIS_TYPE_DOOR, second, MIS_LOC_NONE, false));
         aux = OPEN_SEQ | (strict ? OPEN_STRICT1 : 0u);
       } else if (level == BABYAI_OPENDOORSORDER) {
         rand_colors(arg);
@@ -554,6 +580,10 @@ MG_D void draw_level(const Params &p, Pcg &r, Level &L) {
         m1 = 1u << c[mode == 2 ? i2 : i1];
         if (mode != 0) m2 = 1u << c[mode == 2 ? i1 : i2];
         aux = (mode != 0 ? OPEN_SEQ : 0u) | (strict ? OPEN_STRICT1 | OPEN_STRICT2 : 0u);
+        // the mission keeps the reference's surface order: desc1 is instr_a also in an AfterInstr
+        mis = mission_code(mode == 0 ? MIS_OPEN : mode == 1 ? MIS_BEFORE : MIS_AFTER,
+                           mission_desc(MIS_TYPE_DOOR, c[i1], MIS_LOC_NONE, false),
+                           mode == 0 ? 0u : mission_desc(MIS_TYPE_DOOR, c[i2], MIS_LOC_NONE, false));
       } else {  // UnlockLocal: a locked door (side, then colour drawn), its key, distractors, OpenInstr(ObjDesc("door"))
         const int col = add_door(1, 1, -1, -1, 1, px[0], py[0]);
         add_object(1, 1, 0, col);  // reject_next_to is relative to the default agent position, the middle of room (1, 1)
@@ -566,15 +596,17 @@ MG_D void draw_level(const Params &p, Pcg &r, Level &L) {
         }
         place_agent(1, 1);
         m1 = 0x3Fu;
+        mis = mission_code(MIS_OPEN, mission_desc(MIS_TYPE_DOOR, -1, MIS_LOC_NONE, false), 0u);  // the level's one door
       }
       level_target(L, (int)m1, (int)m2, aux);
+      level_set_mission(L, mis);
     } else if (variant == RG_BABYAI_PICKUP_PUTNEXT) {
       // RoomGridLevel._gen_grid (babyai/core/roomgrid_level.py:119-177) with the gen_mission of OneRoomS* (other.py:329-332),
       // PickupDist (pickup.py:275-290) and PutNextLocal (putnext.py:71-80), then validate_instrs; RejectSampling starts
       // the next attempt from an empty room while the stream continues. As for GoTo, place_obj's RecursionError is not
       // modelled.
       const int level = p.kp[4], nobj = p.kp[5];
-      uint32_t tx = 0, ty = 0, aux = 0;
+      uint32_t tx = 0, ty = 0, aux = 0, mis = 0;
       for (;;) {
         L.rm03 = 0; L.nrooms = 0;
         L.ax = S / 2; L.ay = S / 2; L.adir = 0;
@@ -582,6 +614,7 @@ MG_D void draw_level(const Params &p, Pcg &r, Level &L) {
           const uint32_t o = add_object(0, 0, 1, -1);
           place_agent(0, 0);
           tx = T_KEY + ((o >> 10) & 3u); ty = (o >> 12) & 7u; aux = PICK_TYPE;
+          mis = mission_code(MIS_PICKUP, obj_desc(1, -1), 0u);
           break;
         }
         // PutNextLocal places the agent first; PickupDist's objects are placed around the default room centre
@@ -599,6 +632,7 @@ MG_D void draw_level(const Params &p, Pcg &r, Level &L) {
           const int select_by = rng_integers(r, 0, 3);                // _rand_elem(["type", "color", "both"])
           tx = T_KEY + ((o >> 10) & 3u); ty = (o >> 12) & 7u;
           aux = (select_by == 1 ? 0u : PICK_TYPE) | (select_by == 0 ? 0u : PICK_COLOR) | (p.kp[6] ? PICK_STRICT : 0u);
+          mis = mission_code(MIS_PICKUP, obj_desc(select_by == 1 ? -1 : (int)((o >> 10) & 3u), select_by == 0 ? -1 : (int)((o >> 12) & 7u)), 0u);
           break;
         }
         if (!objs_reachable()) continue;  // RejectSampling("unreachable object at ...")
@@ -610,9 +644,12 @@ MG_D void draw_level(const Params &p, Pcg &r, Level &L) {
         // PutNextInstr(ObjDesc(move), ObjDesc(fixed)): the move object's type and colour, the fixed object's cell code
         tx = T_KEY + ((mv >> 10) & 3u); ty = (mv >> 12) & 7u;
         aux = (T_KEY + ((fo >> 10) & 3u)) | (((fo >> 12) & 7u) << 4);
+        mis = mission_code(MIS_PUTNEXT, obj_desc((int)((mv >> 10) & 3u), (int)((mv >> 12) & 7u)),
+                           obj_desc((int)((fo >> 10) & 3u), (int)((fo >> 12) & 7u)));
         break;
       }
       level_target(L, (int)tx, (int)ty, aux);
+      level_set_mission(L, mis);
     } else if (variant == RG_BABYAI_GOTO) {
       // RoomGridLevel._gen_grid (babyai/core/roomgrid_level.py:119-144): an attempt is RoomGrid._gen_grid (one room: no
       // door draws) and gen_mission (babyai/goto.py:67-78, 133-141, 192-193, 256-260, 333-338, 661-677); RejectSampling
@@ -645,6 +682,7 @@ MG_D void draw_level(const Params &p, Pcg &r, Level &L) {
       }
       // GoToInstr(ObjDesc(type, colour)): the step post-filter compares the front cell with (type, colour)
       level_target(L, (int)(T_KEY + ((tgt >> 10) & 3u)), (int)((tgt >> 12) & 7u), 0u);
+      level_set_mission(L, mission_code(MIS_GOTO, obj_desc((int)((tgt >> 10) & 3u), (int)((tgt >> 12) & 7u)), 0u));
     } else if (rg_obstructed(variant)) {
       // ObstructedMazeEnv._gen_grid (obstructedmaze.py:112-126): door_colors = _rand_subset(COLOR_NAMES, 6), the ball to find
       // is COLOR_NAMES[0] (blue), blocking balls COLOR_NAMES[1] (green), boxes COLOR_NAMES[2] (grey)

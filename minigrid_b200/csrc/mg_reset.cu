@@ -43,6 +43,7 @@ k_reset(Params p, const uint8_t *__restrict__ mask, uint8_t *__restrict__ obs, i
       rec.x |= ((uint32_t)level_tx(L) << 16) | ((uint32_t)level_ty(L) << 24);
       rec.y |= level_aux(L) << 16;
     }
+    if (KIND == KIND_ROOMGRID && p.extra) mission_codes(p)[env] = level_mission(L);
     if (KIND == KIND_DYNOBS) {
       uint32_t ex[4];
       dynobs_pack(L, ex);

@@ -174,6 +174,7 @@ __device__ __noinline__ ResetOut warp_reset(const Params &p, unsigned pend, int 
     Pcg r = load_rng(rr);
     draw_level<KIND>(p, r, L);
     store_rng(rr, r);
+    if (KIND == KIND_ROOMGRID && p.extra) mission_codes(p)[(size_t)tile * TILE + lane] = level_mission(L);  // the new episode's mission
     if (KIND == KIND_DYNOBS) {  // the obstacle list of the new episode
       uint32_t ex[4];
       dynobs_pack(L, ex);

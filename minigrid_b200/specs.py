@@ -326,6 +326,49 @@ BABYAI_OPEN_REGISTRY = {
 }
 
 
+def is_babyai(spec: EnvSpec) -> bool:
+    """A BabyAI level (roomgrid variants 7..9): its mission is the instruction the generator drew."""
+    return spec.kind == KIND_ROOMGRID and len(spec.params) > 0 and spec.params[0] in (BABYAI_GOTO, BABYAI_PICKUP_PUTNEXT, BABYAI_OPEN)
+
+
+_COLORS = frozenset(["red", "green", "blue", "purple", "yellow", "grey"])
+_TYPES = frozenset(["key", "ball", "box"])
+_LOC_WORDS = frozenset(["on", "your", "left", "right", "in", "front", "of", "you", "behind"])  # ObjDesc.surface's loc phrases
+
+
+def babyai_mission_words(spec: EnvSpec) -> frozenset:
+    """Every word the mission grammar of a BabyAI level can produce (the comma counted as a word, as
+    DictObservationSpaceWrapper.string_to_indices splits it): the instructions its gen_mission builds and the ObjDesc
+    surfaces they can take (babyai/core/verifier.py:64-100)."""
+    if not is_babyai(spec):
+        raise ValueError("not a BabyAI level")
+    variant, level, arg = spec.params[0], spec.params[4], spec.params[5]
+    art = {"a", "the"}
+    if variant == BABYAI_GOTO:  # GoToInstr(ObjDesc(type, colour))
+        return frozenset({"go", "to"} | art | _COLORS | _TYPES)
+    if variant == BABYAI_PICKUP_PUTNEXT:
+        if level == BABYAI_ONEROOM:  # PickupInstr(ObjDesc("ball"))
+            return frozenset({"pick", "up", "the", "ball"})
+        if level == BABYAI_PICKUPDIST:  # PickupInstr(ObjDesc(type or None, colour or None))
+            return frozenset({"pick", "up", "object"} | art | _COLORS | _TYPES)
+        return frozenset({"put", "next", "to"} | art | _COLORS | _TYPES)  # PutNextInstr
+    door = {"open", "the", "door"}
+    if level == BABYAI_OPENREDDOOR:
+        return frozenset(door | {"red"})
+    if level == BABYAI_OPENDOOR:  # select_by colour, loc or drawn between them
+        return frozenset(door | (_COLORS if arg != _SELECT_BY["loc"] else set())
+                         | ({"a"} | _LOC_WORDS if arg != _SELECT_BY["color"] else set()))
+    if level == BABYAI_OPENTWODOORS:  # BeforeInstr
+        return frozenset(door | _COLORS | {",", "then"})
+    if level == BABYAI_OPENDOORSORDER:  # OpenInstr, BeforeInstr or AfterInstr
+        return frozenset(door | _COLORS | {",", "then", "after", "you"})
+    return frozenset(door)  # UnlockLocal: OpenInstr(ObjDesc("door"))
+
+
+# the most words (the comma counted) of any BabyAI mission: "open the purple door , then open the yellow door"
+BABYAI_MISSION_MAX_WORDS = 10
+
+
 def get(env_id: str) -> EnvSpec:
     if env_id in BABYAI_REGISTRY:
         return BABYAI_REGISTRY[env_id]

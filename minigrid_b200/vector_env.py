@@ -38,11 +38,16 @@ except Exception:  # noqa: BLE001
 
 class MinigridVecEnv(_VectorEnvBase):
     """Batched MiniGridEnv on one GPU. `seed_offset` is this shard's first global env index (multi-GPU): without an
-    explicit seed, env i starts from seed `seed_offset + i`."""
+    explicit seed, env i starts from seed `seed_offset + i`.
+
+    `missions=True` (BabyAI levels): every reset and autoreset also records the mission it drew, as one code per env on
+    the device (`mission_codes`). `missions()` turns them into the reference's strings, and FlatObsWrapper /
+    DictObservationSpaceWrapper then encode each env's own mission on the device. obs["mission"] stays the spec's
+    template string either way: building num_envs Python strings per step has no place on the step path."""
 
     def __init__(self, env_id: str | None = None, num_envs: int = 1, *, spec: specs.EnvSpec | None = None,
                  device: int | str | torch.device | None = None, autoreset_mode: str = "next_step",
-                 seed_offset: int = 0):
+                 seed_offset: int = 0, missions: bool = False):
         if not torch.cuda.is_available():
             raise _lib.MinigridB200Error("minigrid_b200 needs a CUDA device (H100, sm_90a); there is no CPU path")
         self.level_spec = spec if spec is not None else specs.get(env_id)
@@ -62,6 +67,9 @@ class MinigridVecEnv(_VectorEnvBase):
                                      int(self.level_spec.see_through_walls), prm, len(self.level_spec.params), self.num_envs,
                                      AUTORESET[autoreset_mode], self.device.index, C.byref(h)))
         self._h = h
+        self.missions_enabled = bool(missions)
+        if self.missions_enabled:  # before anything seeds or resets the envs
+            _lib.check(self._L.mg_enable_missions(self._h))
         if self.seed_offset:  # mg_create seeds env i with i: shards of one batch must not hold identical envs
             _lib.check(self._L.mg_seed_base(self._h, C.c_uint64(self.seed_offset), self._stream()))
         n, d = self.num_envs, self.device
@@ -92,6 +100,7 @@ class MinigridVecEnv(_VectorEnvBase):
         self.mission = self.level_spec.mission
         self._obs_dict = {"image": self._image, "direction": self._direction, "mission": self.mission}
         self.width, self.height, self.max_steps = self.level_spec.width, self.level_spec.height, self.level_spec.max_steps
+        self._codes = torch.zeros(n, dtype=torch.int32, device=d) if self.missions_enabled else None
 
     # ---- plumbing ----
     def _stream(self):
@@ -246,6 +255,40 @@ class MinigridVecEnv(_VectorEnvBase):
                                             self._p(hb["reward"]), self._p(hb["terminated"]), self._p(hb["truncated"])))
         obs = {"image": hb["image"], "direction": hb["direction"], "mission": self.mission}
         return obs, hb["reward"], hb["terminated"], hb["truncated"], {}
+
+    # ---- per-episode missions (missions=True) ----
+    @property
+    def mission_codes(self) -> torch.Tensor:
+        """int32[n] on the device: each env's mission code (layout: minigrid_b200/csrc/mg_common.cuh, MIS_*) as the last
+        reset or step left it; copied on the current stream at every access. 0 for a level whose mission is constant."""
+        if not self.missions_enabled:
+            raise ValueError("mission codes need MinigridVecEnv(..., missions=True)")
+        with torch.cuda.device(self.device):
+            _lib.check(self._L.mg_get_mission_codes(self._h, self._p(self._codes), self._stream()))
+        return self._codes
+
+    def mission_text(self, out: torch.Tensor | None = None) -> torch.Tensor:
+        """uint8[n, 96] on the device: every env's mission string, zero padded (BabyAI levels with missions=True)."""
+        self._require_babyai_missions()
+        if out is None:
+            out = torch.empty((self.num_envs, 96), dtype=torch.uint8, device=self.device)
+        with torch.cuda.device(self.device):
+            _lib.check(self._L.mg_mission_text(self._h, self._p(out), self._stream()))
+        return out
+
+    def missions(self) -> list[str]:
+        """[env.mission for every env], as the reference's envs hold it after the last reset or step (synchronises).
+        A level with a constant mission returns the spec's string for every env."""
+        if "{" not in self.mission and not (self.missions_enabled and specs.is_babyai(self.level_spec)):
+            return [self.mission] * self.num_envs
+        txt = self.mission_text().cpu().numpy()
+        return [bytes(row).rstrip(b"\0").decode() for row in txt]
+
+    def _require_babyai_missions(self):
+        if not self.missions_enabled:
+            raise ValueError(f"{self.env_id or 'this level'}: per-episode missions need MinigridVecEnv(..., missions=True)")
+        if not specs.is_babyai(self.level_spec):
+            raise ValueError(f"{self.env_id or 'this level'} is not a BabyAI level: its mission is not encoded per env")
 
     # ---- wrappers' data and state exchange ----
     def full_obs(self, out: torch.Tensor | None = None):

@@ -5,15 +5,18 @@ FullyObsWrapper          :383-426  obs["image"] = grid.encode() with the agent c
                                    COLOR_TO_IDX["red"], agent_dir); shape (W, H, 3) per env.
 ViewSizeWrapper          :629-673  obs["image"] regenerated with another odd agent_view_size (3..15).
 OneHotPartialObsWrapper  :217-284  obs["image"] -> (V, V, 20) one-hot of (type, colour, state).
-FlatObsWrapper           :557-626  uint8[V*V*3 + 28*96]: the image followed by the one-hot mission characters (ids with a
-                                   constant mission string only: the engine does not produce per-episode missions).
+FlatObsWrapper           :557-626  uint8[V*V*3 + 28*96]: the image followed by the one-hot mission characters: the
+                                   constant mission string, or each env's own mission on a BabyAI level created with
+                                   missions=True.
 SymbolicObsWrapper       :729-782  obs["image"] = int64 (W, H, 3): (x, y, type or -1), agent cell = 10.
 RGBImgPartialObsWrapper  :334-380  obs["image"] = the agent's view rendered with 8 x 8 tiles, (56, 56, 3).
 RGBImgObsWrapper         :287-331  obs["image"] = the whole grid rendered, the agent's view highlighted, (8 H, 8 W, 3).
 The two RGB wrappers copy tiles that the reference's own Grid.render_tile drew (data/tile_atlas.npz).
 
 DictObservationSpaceWrapper :428-554 obs["mission"] = the mission's words as indices into the Minigrid vocabulary, padded to
-                                   max_words_in_mission (host side; ids with a constant mission string only).
+                                   max_words_in_mission: a host list for a constant mission string, an int64[n, max_words]
+                                   device tensor on a BabyAI level created with missions=True whose grammar stays inside
+                                   that vocabulary.
 
 Reward wrappers (they act inside the engine's step kernel, because NoDeath decides whether an episode ends):
 NoDeath                  :809-882  a terminated step into / on a death cell continues with reward + death_cost.
@@ -28,7 +31,7 @@ import os
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, specs
 
 
 class _VecWrapper:
@@ -164,11 +167,22 @@ class OneHotPartialObsWrapper(_DeviceObsWrapper):
         return {**obs, "image": self._out}
 
 
+def _per_env_missions(b) -> bool:
+    """The wrapped env is a BabyAI level whose handle records each env's mission (MinigridVecEnv(..., missions=True))."""
+    return bool(getattr(b, "missions_enabled", False)) and specs.is_babyai(b.level_spec)
+
+
 class FlatObsWrapper(_DeviceObsWrapper):
     def __init__(self, env, maxStrLen=96):
         super().__init__(env)
         b = self._base()
         mission = b.mission
+        self._per_env = _per_env_missions(b)
+        if self._per_env:  # each env's own mission, one-hot encoded on the device (mg_obs_flat_missions)
+            if maxStrLen != 96:
+                raise ValueError("per-env missions are encoded with maxStrLen = 96 (the wrapper's default)")
+            self.maxStrLen, self._out = maxStrLen, None
+            return
         if "{" in mission:
             raise ValueError(f"FlatObsWrapper needs a constant mission string; {b.env_id} draws its mission per episode")
         if len(mission) > maxStrLen:
@@ -190,6 +204,11 @@ class FlatObsWrapper(_DeviceObsWrapper):
     def observation(self, obs):
         img = obs["image"].contiguous()
         nb = int(np.prod(img.shape[1:]))
+        if self._per_env:
+            if self._out is None or self._out.shape[1] != nb + 28 * 96:
+                self._out = torch.empty((img.shape[0], nb + 28 * 96), dtype=torch.uint8, device=img.device)
+            self._call(_lib.load().mg_obs_flat_missions, self._p(img), nb, self._p(self._out))
+            return self._out
         if self._out is None or self._out.shape[1] != nb + self._mission.numel():
             self._out = torch.empty((img.shape[0], nb + self._mission.numel()), dtype=torch.uint8, device=img.device)
         self._call(_lib.load().mg_obs_flat, self._p(img), nb, self._p(self._mission), int(self._mission.numel()), self._p(self._out))
@@ -215,13 +234,28 @@ def mission_to_indices(mission: str, max_words_in_mission: int = 50, word_dict=N
     return idx + [0] * (max_words_in_mission - len(idx))
 
 
-class DictObservationSpaceWrapper(_VecWrapper):
-    """obs["mission"] as a fixed-length list of vocabulary indices (the same list for every env of the batch: the engine
-    serves ids whose mission string is constant; the others draw it per episode and are refused here)."""
+class DictObservationSpaceWrapper(_DeviceObsWrapper):
+    """obs["mission"] as a fixed-length list of vocabulary indices: the same list for every env of the batch when the
+    mission string is constant; on a BabyAI level created with missions=True, an int64[n, max_words_in_mission] device
+    tensor with each env's own mission. Refused: ids that draw their mission without missions=True, and BabyAI levels
+    whose grammar has words outside the vocabulary (the reference raises "Unknown word" on those episodes)."""
 
     def __init__(self, env, max_words_in_mission=50, word_dict=None):
         super().__init__(env)
         b = self.unwrapped
+        self._per_env = _per_env_missions(b)
+        if self._per_env:
+            unknown = sorted(specs.babyai_mission_words(b.level_spec) - set(MINIGRID_WORDS))
+            if unknown:
+                raise ValueError(f"{b.env_id}: its missions can contain words outside the Minigrid vocabulary ({', '.join(unknown)})")
+            if word_dict is not None:
+                raise ValueError("per-env missions are encoded with the Minigrid vocabulary (word_dict=None)")
+            if max_words_in_mission <= specs.BABYAI_MISSION_MAX_WORDS:
+                raise ValueError(f"max_words_in_mission must exceed {specs.BABYAI_MISSION_MAX_WORDS}, the longest BabyAI mission")
+            self.max_words_in_mission = max_words_in_mission
+            self.word_dict = {w: i for i, w in enumerate(MINIGRID_WORDS)}
+            self._out = torch.empty((b.num_envs, max_words_in_mission), dtype=torch.int64, device=b.device)
+            return
         if "{" in b.mission:
             raise ValueError(f"DictObservationSpaceWrapper needs a constant mission string; {b.env_id} draws its mission per episode")
         self.max_words_in_mission = max_words_in_mission
@@ -229,6 +263,9 @@ class DictObservationSpaceWrapper(_VecWrapper):
         self._mission = mission_to_indices(b.mission, max_words_in_mission, self.word_dict)
 
     def observation(self, obs):
+        if self._per_env:
+            self._call(_lib.load().mg_mission_indices, self.max_words_in_mission, self._p(self._out))
+            return {**obs, "mission": self._out}
         return {**obs, "mission": list(self._mission)}
 
 
