@@ -76,7 +76,13 @@ extern "C" {
                                    colour, 1 loc, 2 drawn), OpenTwoDoors' fixed red / blue colours (0 or 1), OpenDoorsOrder's
                                    num_doors (2..4) or UnlockLocal's distractors (0 or 1), 0 for OpenRedDoor; strict is the
                                    Debug ids' flag (never on OpenRedDoor or UnlockLocal); max_steps is room_size^2 rows cols,
-                                   or 720 for OpenTwoDoors and OpenDoorsOrder, for the registered ids */
+                                   or 720 for OpenTwoDoors and OpenDoorsOrder, for the registered ids;
+                                   envs/babyai/goto.py (GoToObjMaze*), other.py (FindObjS*, KeyCorridor*): {10, room_size,
+                                   num_rows, num_cols, level (0 GoToObjMaze, 1 FindObj, 2 KeyCorridor), arg} with
+                                   room_size 4..8 for GoToObjMaze and FindObj, a square grid of at least 2 x 2 rooms for
+                                   FindObj and 3 columns for KeyCorridor; arg is GoToObjMaze's doors_open (0 or 1), 0
+                                   otherwise; max_steps is room_size^2 rows cols (GoToObjMaze), 20 room_size^2 (FindObj)
+                                   or 30 room_size^2 (KeyCorridor) for the registered ids */
 #define MG_KIND_DYNOBS 15       /* envs/dynamicobstacles.py: params {n_obstacles, random_start, start_x, start_y, start_dir} */
 
 /* gymnasium.vector.AutoresetMode */

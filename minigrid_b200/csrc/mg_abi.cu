@@ -149,10 +149,10 @@ int mg_create(int kind, int width, int height, int max_steps, int see_through_wa
   if (kind == MG_KIND_ROOMGRID) {
     // BabyAI OneRoom is the one level whose room may be larger than 8: it has no reachability fill (a 64-bit mask)
     const bool one_room = n_params >= 5 && params[0] == RG_BABYAI_PICKUP_PUTNEXT && params[4] == BABYAI_ONEROOM;
-    if (n_params < 4 || params[0] < 0 || params[0] > RG_BABYAI_OPEN || params[1] < 3 || params[1] > (one_room ? 20 : 8) ||
+    if (n_params < 4 || params[0] < 0 || params[0] > RG_BABYAI_MAZE || params[1] < 3 || params[1] > (one_room ? 20 : 8) ||
         params[2] < 1 || params[3] < 1 || params[2] * params[3] > 9 || width != (params[1] - 1) * params[3] + 1 ||
         height != (params[1] - 1) * params[2] + 1)
-      return fail(MG_ERR_INVALID_ARG, "roomgrid needs params {variant 0..9, room_size 3..8 (..20 for BabyAI OneRoom), num_rows, num_cols} "
+      return fail(MG_ERR_INVALID_ARG, "roomgrid needs params {variant 0..10, room_size 3..8 (..20 for BabyAI OneRoom), num_rows, num_cols} "
                                       "with at most 9 rooms, width = (room_size - 1) num_cols + 1 and height = (room_size - 1) num_rows + 1 "
                                       "(roomgrid.py:83-84)");
     if (params[0] == 3 && params[3] != 3) return fail(MG_ERR_INVALID_ARG, "keycorridor has 3 columns of rooms (keycorridor.py:104-126)");
@@ -201,6 +201,22 @@ int mg_create(int kind, int width, int height, int max_steps, int see_through_wa
                                         "fixed red / blue 0 or 1 for OpenTwoDoors, num_doors 2..4 for OpenDoorsOrder and "
                                         "distractors 0 or 1 for UnlockLocal (0 for OpenRedDoor); strict 0 or 1, and 0 for "
                                         "OpenRedDoor and UnlockLocal");
+    }
+    if (params[0] == RG_BABYAI_MAZE) {
+      // GoTo places the agent in any room, then its object in any room away from the agent: a room of 4 keeps one such
+      // cell, a room of 3 none. FindObj draws the object's room i from num_rows and j from num_cols and places the agent
+      // in room (1, 1), so its grid is square with at least 2 x 2 rooms. KeyCorridor is MiniGrid's, 3 columns. A seventh
+      // parameter (the strict flag of variants 8 and 9) means nothing here and is refused rather than ignored.
+      const int S = params[1], rows = params[2], cols = params[3];
+      const int level = n_params == 6 ? params[4] : -1, arg = n_params == 6 ? params[5] : -1;
+      const bool ok = level == BABYAI_MAZE_GOTO ? (S >= 4 && (arg == 0 || arg == 1))
+                      : level == BABYAI_FINDOBJ ? (S >= 4 && rows == cols && rows >= 2 && arg == 0)
+                      : level == BABYAI_MAZE_KEYCORRIDOR && cols == 3 && arg == 0;
+      if (n_params != 6 || !ok)
+        return fail(MG_ERR_INVALID_ARG, "babyai maze needs exactly params {10, room_size, num_rows, num_cols, level 0..2 (GoToObjMaze, "
+                                        "FindObj, KeyCorridor), arg}: room_size 4..8 for GoToObjMaze and FindObj, square with at "
+                                        "least 2 x 2 rooms for FindObj, 3 columns for KeyCorridor; arg is doors_open 0 or 1 for "
+                                        "GoToObjMaze and 0 otherwise");
     }
     if (rg_obstructed(params[0])) {
       if (n_params < 8 || params[1] < 4) return fail(MG_ERR_INVALID_ARG, "obstructedmaze needs params {variant, room_size >= 4, num_rows, num_cols, key_in_box, blocked, agent_room_i | agent_room_j << 4, num_quarters}");

@@ -88,7 +88,10 @@ enum : int { RG_UNLOCK = 0, RG_UNLOCKPICKUP = 1, RG_BLOCKEDUNLOCKPICKUP = 2, RG_
              RG_BABYAI_PICKUP_PUTNEXT = 8,
              // the BabyAI Open and UnlockLocal levels (envs/babyai/open.py, unlock.py):
              // kp = {9, room_size, num_rows, num_cols, level, arg, strict}
-             RG_BABYAI_OPEN = 9 };  // kinds mg_create accepts: the kernels are instantiated for the kinds below this
+             RG_BABYAI_OPEN = 9,
+             // the BabyAI levels that span a maze of rooms joined by connect_all (envs/babyai/goto.py GoTo with one
+             // object, other.py FindObjS5 and KeyCorridor): kp = {10, room_size, num_rows, num_cols, level, arg}
+             RG_BABYAI_MAZE = 10 };  // kinds mg_create accepts: the kernels are instantiated for the kinds below this
 MG_HD bool rg_obstructed(int variant) { return variant >= RG_OBSTRUCTED_1D && variant <= RG_OBSTRUCTED_FULL_V1; }
 // kp[4] of RG_BABYAI_GOTO: GoToRedBallGrey, GoToRedBall(NoDists), GoToObj, GoToLocal, GoToRedBlueBall
 enum : int { BABYAI_REDBALL_GREY = 0, BABYAI_REDBALL = 1, BABYAI_OBJ = 2, BABYAI_LOCAL = 3, BABYAI_REDBLUEBALL = 4 };
@@ -105,6 +108,12 @@ enum : int { BABYAI_OPENREDDOOR = 0, BABYAI_OPENDOOR = 1, BABYAI_OPENTWODOORS = 
 // AfterInstr is stored with its two instructions swapped), OPEN_STRICT1 / 2: their strict flags; OPEN_DONE: the first
 // has succeeded (BeforeInstr.a_done / AfterInstr.b_done), the one bit K1 changes during an episode
 enum : uint32_t { OPEN_SEQ = 1u, OPEN_STRICT1 = 2u, OPEN_STRICT2 = 4u, OPEN_DONE = 8u };
+// kp[4] of RG_BABYAI_MAZE: GoToObjMaze* (kp[5] = doors_open), FindObjS*, KeyCorridor* (MiniGrid KeyCorridor's generator)
+enum : int { BABYAI_MAZE_GOTO = 0, BABYAI_FINDOBJ = 1, BABYAI_MAZE_KEYCORRIDOR = 2 };
+// KeyCorridor's generator: the MiniGrid level, or the BabyAI level that makes the same draws
+MG_HD bool rg_keycorridor(const int *kp) {
+  return kp[0] == RG_KEYCORRIDOR || (kp[0] == RG_BABYAI_MAZE && kp[4] == BABYAI_MAZE_KEYCORRIDOR);
+}
 // Mission code of a BabyAI level (Params::mission, one word per env, written by every reset when the handle asked for
 // missions): the instruction that RoomGridLevel._gen_grid turns into self.mission = self.instrs.surface(self)
 // (babyai/core/roomgrid_level.py:142-144), rendered back into text by mission_words (mg_mission.cuh).

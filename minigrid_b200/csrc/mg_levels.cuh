@@ -262,17 +262,21 @@ MG_D uint32_t rg_door_code(uint32_t dsc) {
 MG_D uint32_t cell_roomgrid(const Geom &g, const int *kp, const Level &L, int x, int y) {
   const int S1 = kp[1] - 1, cols = kp[3];
   const int i = x / S1, j = y / S1, lx = x - i * S1, ly = y - j * S1;
+  // GoToObjMazeOpen: open_all_doors() ends the generator; no draw reads a door's state
+  const bool doors_open = kp[0] == RG_BABYAI_MAZE && kp[4] == BABYAI_MAZE_GOTO && kp[5];
   if (lx == 0 && ly == 0) return CODE_WALL;
   if (lx == 0) {  // the vertical wall left of room (i, j) = right of room (i - 1, j)
     if (i == 0 || x == g.W - 1) return CODE_WALL;
     const uint32_t dsc = rg_vdoor(L, j * (cols - 1) + (i - 1));
-    return ((dsc & 0x80u) && ly - 1 == (int)(dsc & 7u)) ? rg_door_code(dsc) : CODE_WALL;
+    if (!(dsc & 0x80u) || ly - 1 != (int)(dsc & 7u)) return CODE_WALL;
+    return doors_open ? (T_DOOR | (((dsc >> 3) & 7u) << 4)) : rg_door_code(dsc);
   }
   if (ly == 0) {  // the horizontal wall above room (i, j) = below room (i, j - 1)
     if (j == 0 || y == g.H - 1) return CODE_WALL;
-    if (kp[0] == RG_KEYCORRIDOR && i == 1) return CODE_EMPTY;  // remove_wall(1, j, 3), j >= 1
+    if (rg_keycorridor(kp) && i == 1) return CODE_EMPTY;  // remove_wall(1, j, 3), j >= 1
     const uint32_t dsc = rg_hdoor(L, (j - 1) * cols + i);
-    return ((dsc & 0x80u) && lx - 1 == (int)(dsc & 7u)) ? rg_door_code(dsc) : CODE_WALL;
+    if (!(dsc & 0x80u) || lx - 1 != (int)(dsc & 7u)) return CODE_WALL;
+    return doors_open ? (T_DOOR | (((dsc >> 3) & 7u) << 4)) : rg_door_code(dsc);
   }
   if (rg_obstructed(kp[0]) && x == L.e && y == L.f) return T_BALL | (C_BLUE << 4);  // self.obj: COLOR_NAMES[0]
   // the objects in creation order; a later grid.set wins (ObstructedMaze v0 puts blocking balls over earlier keys)
@@ -416,14 +420,19 @@ MG_D void draw_level(const Params &p, Pcg &r, Level &L) {
     // RoomGrid._gen_grid (roomgrid.py:123-177), then the env's own _gen_grid (unlock.py:72-84, unlockpickup.py:80-93,
     // blockedunlockpickup.py:87-103, keycorridor.py:104-126) with RoomGrid's helpers restated as lambdas
     const int variant = p.kp[0], S = p.kp[1], rows = p.kp[2], cols = p.kp[3], S1 = S - 1;
-    for (int j = 0; j < rows; ++j)
-      for (int i = 0; i < cols; ++i) {  // door_pos draws: right wall (y), then bottom wall (x)
-        if (i < cols - 1) L.oh |= (unsigned long long)rng_integers(r, 0, S - 2) << (8 * (j * (cols - 1) + i));
-        if (j < rows - 1) L.rm45 |= (unsigned long long)rng_integers(r, 0, S - 2) << (8 * (j * cols + i));
-      }
-    L.ax = (cols / 2) * S1 + S / 2; L.ay = (rows / 2) * S1 + S / 2; L.adir = 0;  // "the agent starts in the middle, facing right"
     unsigned long long conn = 0;  // Room.doors[k] is truthy: bit 4 q + k of room q = j cols + i (k: right, down, left, up)
     uint32_t locked_rooms = 0;    // Room.locked
+    auto room_grid = [&]() {  // an empty grid of rooms, new door positions, the agent's default cell
+      L.oh = 0; L.rm45 = 0; L.rm03 = 0; L.rmx = 0; L.nrooms = 0;
+      conn = 0; locked_rooms = 0;
+      for (int j = 0; j < rows; ++j)
+        for (int i = 0; i < cols; ++i) {  // door_pos draws: right wall (y), then bottom wall (x)
+          if (i < cols - 1) L.oh |= (unsigned long long)rng_integers(r, 0, S - 2) << (8 * (j * (cols - 1) + i));
+          if (j < rows - 1) L.rm45 |= (unsigned long long)rng_integers(r, 0, S - 2) << (8 * (j * cols + i));
+        }
+      L.ax = (cols / 2) * S1 + S / 2; L.ay = (rows / 2) * S1 + S / 2; L.adir = 0;  // "the agent starts in the middle, facing right"
+    };
+    room_grid();
     auto nbr = [&](int i, int j, int k, int &ni, int &nj) -> bool {
       ni = i + (k == 0) - (k == 2); nj = j + (k == 1) - (k == 3);
       return ni >= 0 && ni < cols && nj >= 0 && nj < rows;
@@ -515,6 +524,88 @@ MG_D void draw_level(const Params &p, Pcg &r, Level &L) {
     // ObjDesc(kind, colour) of the mission code, "a" when several cells match it
     auto obj_desc = [&](int kind, int color) -> uint32_t {
       return mission_desc(kind < 0 ? MIS_TYPE_NONE : MIS_TYPE_KEY + (uint32_t)kind, color, MIS_LOC_NONE, n_matching(kind, color) > 1);
+    };
+    // connect_all (roomgrid.py:337-393): random doors until every room is reachable from the agent's. Each try draws
+    // i, j, k; a wall without door_pos, an existing door or a locked room on either side is skipped before the colour
+    // is drawn. The RecursionError after 5000 tries is not modelled: every room here can get a door on every wall.
+    auto connect_all = [&]() {
+      const int start = (L.ay / S1) * cols + (L.ax / S1);
+      for (;;) {
+        uint32_t reach = 0, stack = 1u << start;
+        while (stack) {
+          const int q = __ffs(stack) - 1;
+          stack &= stack - 1;
+          if ((reach >> q) & 1u) continue;
+          reach |= 1u << q;
+          for (int k = 0; k < 4; ++k) {
+            int ni, nj;
+            if (((conn >> (4 * q + k)) & 1ull) && nbr(q % cols, q / cols, k, ni, nj)) stack |= 1u << (nj * cols + ni);
+          }
+        }
+        if (__popc(reach) == rows * cols) break;
+        const int i = rng_integers(r, 0, cols), j = rng_integers(r, 0, rows), k = rng_integers(r, 0, 4);
+        int ni, nj;
+        if (!nbr(i, j, k, ni, nj) || ((conn >> (4 * (j * cols + i) + k)) & 1ull)) continue;  // no door_pos there, or already a door
+        if (((locked_rooms >> (j * cols + i)) & 1u) || ((locked_rooms >> (nj * cols + ni)) & 1u)) continue;
+        const int color = (int)color_name_idx(rng_integers(r, 0, 6));
+        int qx, qy;
+        add_door(i, j, k, color, 0, qx, qy);
+      }
+    };
+    // check_objs_reachable (roomgrid_level.py:250-302) over a grid of rooms, up to 22 x 22 cells: flood fill from the
+    // agent through empty cells and doors in any state; an object cell is reached but stops the fill; false when an
+    // object or a door is not reached. Bit x of row word y; `live` holds the reached cells the fill goes on from, and a
+    // row is closed horizontally in one step: for seeds s inside the passable cells e, ((e + s) ^ e) | s is every cell
+    // from the lowest seed of a run of e up to the first cell past it (the carry runs through the run), and the same on
+    // the bit-reversed words gives the other direction. The one-room levels keep objs_reachable: its grid is one 64-bit
+    // word in registers, where this one walks an array of rows.
+    auto maze_reachable = [&]() -> bool {
+      uint32_t inner = 0;  // the columns that are not a vertical wall line
+      for (int x = 0; x < W; ++x) inner |= (x % S1 != 0 ? 1u : 0u) << x;
+      auto row_masks = [&](int y, uint32_t &ext, uint32_t &tgt) {  // ext: empty cells and doors; tgt: objects and doors
+        const int j = y / S1, ly = y - j * S1;
+        uint32_t doors = 0, objs = 0, open = 0;
+        if (ly == 0) {
+          if (j > 0 && j < rows)
+            for (int i = 0; i < cols; ++i) {
+              const uint32_t dsc = rg_hdoor(L, (j - 1) * cols + i);
+              if (dsc & 0x80u) doors |= 1u << (i * S1 + 1 + (int)(dsc & 7u));
+            }
+        } else {
+          for (int i = 1; i < cols; ++i) {
+            const uint32_t dsc = rg_vdoor(L, j * (cols - 1) + (i - 1));
+            if ((dsc & 0x80u) && ly - 1 == (int)(dsc & 7u)) doors |= 1u << (i * S1);
+          }
+          for (int k = 0; k < L.nrooms; ++k) {
+            const uint32_t o = rg_obj(L, k);
+            if ((int)((o >> 5) & 31u) == y) objs |= 1u << (o & 31u);
+          }
+          open = inner & ~objs;
+        }
+        ext = open | doors;
+        tgt = objs | doors;
+      };
+      uint32_t live[MAX_DIM];
+      for (int y = 0; y < H; ++y) live[y] = 0;
+      live[L.ay] = 1u << L.ax;
+      for (bool changed = true; changed;) {
+        changed = false;
+        for (int y = 1; y < H - 1; ++y) {
+          uint32_t ext, tgt;
+          row_masks(y, ext, tgt);
+          const uint32_t s = (live[y] | live[y - 1] | live[y + 1]) & ext;
+          const uint32_t sr = __brev(s), er = __brev(ext);
+          const uint32_t fill = (((ext + s) ^ ext) | s | __brev(((er + sr) ^ er) | sr)) & ext;
+          if (fill != live[y]) { live[y] = fill; changed = true; }
+        }
+      }
+      for (int y = 1; y < H - 1; ++y) {
+        uint32_t ext, tgt;
+        row_masks(y, ext, tgt);
+        const uint32_t reached = live[y] | (live[y] << 1) | (live[y] >> 1) | live[y - 1] | live[y + 1];
+        if (tgt & ~reached) return false;
+      }
+      return true;
     };
     int dpx = 0, dpy = 0;
     if (variant == RG_BABYAI_OPEN) {
@@ -733,7 +824,8 @@ MG_D void draw_level(const Params &p, Pcg &r, Level &L) {
         place_agent(p.kp[6] & 15, p.kp[6] >> 4);
       }
       level_target(L, (int)T_BALL, (int)C_BLUE, 0u);
-    } else if (variant == RG_KEYCORRIDOR) {
+    } else if (rg_keycorridor(p.kp)) {
+      // keycorridor.py:104-126; BabyAI's KeyCorridor (babyai/other.py:252-272) makes the same draws
       for (int j = 1; j < rows; ++j) {  // remove_wall(1, j, 3): the cells are handled by cell_roomgrid, the rooms become connected
         conn |= 1ull << (4 * (j * cols + 1) + 3);
         conn |= 1ull << (4 * ((j - 1) * cols + 1) + 1);
@@ -744,30 +836,43 @@ MG_D void draw_level(const Params &p, Pcg &r, Level &L) {
       const int key_row = rng_integers(r, 0, rows);
       add_object(0, key_row, 0, door_color);
       place_agent(1, rows / 2);
-      // connect_all (roomgrid.py:337-393): random doors until every room is reachable from the agent's
-      const int start = (L.ay / S1) * cols + (L.ax / S1);
-      for (;;) {
-        uint32_t reach = 0, stack = 1u << start;
-        while (stack) {
-          const int q = __ffs(stack) - 1;
-          stack &= stack - 1;
-          if ((reach >> q) & 1u) continue;
-          reach |= 1u << q;
-          for (int k = 0; k < 4; ++k) {
-            int ni, nj;
-            if (((conn >> (4 * q + k)) & 1ull) && nbr(q % cols, q / cols, k, ni, nj)) stack |= 1u << (nj * cols + ni);
-          }
-        }
-        if (__popc(reach) == rows * cols) break;
-        const int i = rng_integers(r, 0, cols), j = rng_integers(r, 0, rows), k = rng_integers(r, 0, 4);
-        int ni, nj;
-        if (!nbr(i, j, k, ni, nj) || ((conn >> (4 * (j * cols + i) + k)) & 1ull)) continue;  // no door_pos there, or already a door
-        if (((locked_rooms >> (j * cols + i)) & 1u) || ((locked_rooms >> (nj * cols + ni)) & 1u)) continue;
-        const int color = (int)color_name_idx(rng_integers(r, 0, 6));
-        int qx, qy;
-        add_door(i, j, k, color, 0, qx, qy);
+      connect_all();
+      if (variant == RG_KEYCORRIDOR) {
+        level_target(L, (int)(T_KEY + ((obj >> 10) & 3u)), (int)((obj >> 12) & 7u), 0u);
+      } else {  // PickupInstr(ObjDesc("ball")): the level's one ball
+        level_target(L, (int)T_BALL, 0, PICK_TYPE);
+        level_set_mission(L, mission_code(MIS_PICKUP, mission_desc(MIS_TYPE_BALL, -1, MIS_LOC_NONE, false), 0u));
       }
-      level_target(L, (int)(T_KEY + ((obj >> 10) & 3u)), (int)((obj >> 12) & 7u), 0u);
+    } else if (variant == RG_BABYAI_MAZE) {
+      // RoomGridLevel._gen_grid (babyai/core/roomgrid_level.py:119-144) with the gen_mission of GoTo with one object
+      // (goto.py:416-426) and FindObjS5 (other.py:169-177). A GoTo rejection starts again from RoomGrid._gen_grid: new
+      // door positions, no doors or objects, the default agent cell. FindObj never rejects.
+      uint32_t o;
+      if (p.kp[4] == BABYAI_FINDOBJ) {
+        const int oi = rng_integers(r, 0, rows), oj = rng_integers(r, 0, cols);  // i from num_rows, j from num_cols
+        o = add_object(oi, oj, -1, -1);  // kind, then colour; away from the default agent cell in room (1, 1)
+        place_agent(1, 1);
+        connect_all();
+        level_target(L, (int)(T_KEY + ((o >> 10) & 3u)), 0, PICK_TYPE);  // PickupInstr(ObjDesc(obj.type))
+        level_set_mission(L, mission_code(MIS_PICKUP, mission_desc(MIS_TYPE_KEY + ((o >> 10) & 3u), -1, MIS_LOC_NONE, false), 0u));
+      } else {
+        for (;;) {
+          const int ai = rng_integers(r, 0, cols), aj = rng_integers(r, 0, rows);  // place_agent(): i, then j
+          place_agent(ai, aj);
+          connect_all();
+          // add_distractors(num_distractors=1, all_unique=False): colour, type, then the room i, j
+          const int col = (int)color_name_idx(rng_integers(r, 0, 6));
+          const int kind = rng_integers(r, 0, 3);
+          const int oi = rng_integers(r, 0, cols), oj = rng_integers(r, 0, rows);
+          o = add_object(oi, oj, kind, col);
+          if (maze_reachable()) break;  // _rand_elem(objs) of one object draws nothing
+          room_grid();  // RejectSampling("unreachable object at ...")
+        }
+        // GoToInstr(ObjDesc(type, colour)): one object, so "the"; the step post-filter compares the front cell
+        level_target(L, (int)(T_KEY + ((o >> 10) & 3u)), (int)((o >> 12) & 7u), 0u);
+        level_set_mission(L, mission_code(MIS_GOTO, mission_desc(MIS_TYPE_KEY + ((o >> 10) & 3u), (int)((o >> 12) & 7u),
+                                                                 MIS_LOC_NONE, false), 0u));
+      }
     } else {
       uint32_t obj = 0;
       if (variant != RG_UNLOCK) obj = add_object(1, 0, 2, -1);  // a box in the room on the right

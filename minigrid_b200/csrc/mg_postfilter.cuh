@@ -81,17 +81,18 @@ MG_HD PostOut post_filter(const PostIn &in, uint32_t terminated) {
     if (in.ax == in.tx && in.ay == in.ty) { o.reward = POST_REWARD; o.terminated = 1u; }
     if (in.ax == (int)(in.aux & 255u) && in.ay == (int)((in.aux >> 8) & 255u)) { o.reward = POST_ZERO; o.terminated = 1u; }
   } else if (KIND == KIND_ROOMGRID) {
-    if (in.variant == RG_BABYAI_GOTO) {
+    if (in.variant == RG_BABYAI_GOTO || (in.variant == RG_BABYAI_MAZE && in.level == BABYAI_MAZE_GOTO)) {
       // RoomGridLevel.step (babyai/core/roomgrid_level.py:87-104) with GoToInstr.verify_action (verifier.py:290-316):
       // success when front_pos is one of the positions find_matching_objs recorded at reset. A matching object leaves
       // its cell only by being picked up, which needs the agent to face it first, and facing it already ended the
       // episode; so the test is "the front cell holds an object of the target's type and colour" (tx, ty).
       if ((int)(in.front & 15u) == in.tx && (int)((in.front >> 4) & 7u) == in.ty) { o.reward = POST_REWARD; o.terminated = 1u; }
-    } else if (in.variant == RG_BABYAI_PICKUP_PUTNEXT) {
+    } else if (in.variant == RG_BABYAI_PICKUP_PUTNEXT || in.variant == RG_BABYAI_MAZE) {
+      // FindObj and BabyAI KeyCorridor: PickupInstr(ObjDesc(type)), matched on the type (aux = PICK_TYPE)
       // RoomGridLevel.step (babyai/core/roomgrid_level.py:87-104). The verifiers' preCarrying is what was carried after
       // the previous step: carry_before. No object appears or changes colour in these rooms (a box can only vanish, by
       // toggle), so "is one of obj_set" is "matches the descriptor", and an object is identified by its cell code.
-      if (in.level == BABYAI_PUTNEXTLOCAL) {
+      if (in.variant == RG_BABYAI_PICKUP_PUTNEXT && in.level == BABYAI_PUTNEXTLOCAL) {
         // PutNextInstr.verify_action (verifier.py:411-435) after update_objs_poss on a drop: success when preCarrying is
         // the move object and its cur_pos is 4-adjacent to where the fixed object (cell code aux) is now. A drop that
         // failed leaves cur_pos = (-1, -1) from the pickup; one that succeeded put it in the front cell, and the fixed

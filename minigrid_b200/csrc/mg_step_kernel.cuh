@@ -580,7 +580,8 @@ k_step(const __grid_constant__ Params p, const void *__restrict__ actions, int a
         in.red_before = in.blue_before = in.red_after = in.blue_after = false;
         in.variant = p.kp[0]; in.door_open = false; in.front = 0;
         // the front cell after this step's turn, move or mutation (GoTo on every step, Open on a toggle)
-        if (KIND == KIND_ROOMGRID && (p.kp[0] == RG_BABYAI_GOTO || (p.kp[0] == RG_BABYAI_OPEN && act == A_TOGGLE))) {
+        if (KIND == KIND_ROOMGRID && (p.kp[0] == RG_BABYAI_GOTO || (p.kp[0] == RG_BABYAI_MAZE && p.kp[4] == BABYAI_MAZE_GOTO) ||
+                                      (p.kp[0] == RG_BABYAI_OPEN && act == A_TOGGLE))) {
           if (WIN) {  // the loaded words hold the agent's line for its new direction, the mutation included
             in.front = view_words_byte(vw, ((dir & 1) ? ay : ax) + ((dir < 2) ? 1 : -1));
           } else {

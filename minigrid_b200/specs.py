@@ -326,9 +326,40 @@ BABYAI_OPEN_REGISTRY = {
 }
 
 
+BABYAI_MAZE = 10  # roomgrid variant of the BabyAI levels that connect a maze of rooms
+BABYAI_MAZE_GOTO, BABYAI_FINDOBJ, BABYAI_MAZE_KEYCORRIDOR = 0, 1, 2
+
+
+def babyai_maze(level, room_size, num_rows, num_cols, max_steps, mission, arg=0):
+    """envs/babyai/goto.py (GoTo with one object; arg = doors_open) and other.py (FindObjS5, KeyCorridor)."""
+    return roomgrid(BABYAI_MAZE, room_size, num_rows, num_cols, max_steps, mission, (level, int(arg)))
+
+
+def _goto_obj_maze(room_size=8, num_rows=3, num_cols=3, doors_open=False):
+    """max_steps = room_size^2 rows cols: one navigation (roomgrid_level.py:71-85)"""
+    return babyai_maze(BABYAI_MAZE_GOTO, room_size, num_rows, num_cols, room_size * room_size * num_rows * num_cols,
+                       "go to the {color} {type}", doors_open)
+
+
+# __init__.py:692-732, 1001-1057 (the BabyAI levels with connect_all and at most two objects). BabyAI's KeyCorridor makes
+# MiniGrid KeyCorridor's draws; its mission does not name the ball's colour.
+BABYAI_MAZE_REGISTRY = {
+    "BabyAI-GoToObjMaze-v0": _goto_obj_maze(),
+    "BabyAI-GoToObjMazeOpen-v0": _goto_obj_maze(doors_open=True),
+    "BabyAI-GoToObjMazeS4R2-v0": _goto_obj_maze(4, 2, 2),
+    **{f"BabyAI-GoToObjMazeS{s}-v0": _goto_obj_maze(s) for s in (4, 5, 6, 7)},
+    **{f"BabyAI-FindObjS{s}-v0": babyai_maze(BABYAI_FINDOBJ, s, 3, 3, 20 * s * s, "pick up the {type}")
+       for s in (5, 6, 7)},
+    "BabyAI-KeyCorridor-v0": babyai_maze(BABYAI_MAZE_KEYCORRIDOR, 6, 3, 3, 30 * 36, "pick up the ball"),
+    **{f"BabyAI-KeyCorridorS{s}R{r}-v0": babyai_maze(BABYAI_MAZE_KEYCORRIDOR, s, r, 3, 30 * s * s, "pick up the ball")
+       for s, r in [(3, 1), (3, 2), (3, 3), (4, 3), (5, 3), (6, 3)]},
+}
+
+
 def is_babyai(spec: EnvSpec) -> bool:
-    """A BabyAI level (roomgrid variants 7..9): its mission is the instruction the generator drew."""
-    return spec.kind == KIND_ROOMGRID and len(spec.params) > 0 and spec.params[0] in (BABYAI_GOTO, BABYAI_PICKUP_PUTNEXT, BABYAI_OPEN)
+    """A BabyAI level (roomgrid variants 7..10): its mission is the instruction the generator drew."""
+    return spec.kind == KIND_ROOMGRID and len(spec.params) > 0 and spec.params[0] in (BABYAI_GOTO, BABYAI_PICKUP_PUTNEXT,
+                                                                                       BABYAI_OPEN, BABYAI_MAZE)
 
 
 _COLORS = frozenset(["red", "green", "blue", "purple", "yellow", "grey"])
@@ -344,6 +375,10 @@ def babyai_mission_words(spec: EnvSpec) -> frozenset:
         raise ValueError("not a BabyAI level")
     variant, level, arg = spec.params[0], spec.params[4], spec.params[5]
     art = {"a", "the"}
+    if variant == BABYAI_MAZE:  # one object: GoToInstr(ObjDesc(type, colour)) or PickupInstr(ObjDesc(type))
+        if level == BABYAI_MAZE_GOTO:
+            return frozenset({"go", "to", "the"} | _COLORS | _TYPES)
+        return frozenset({"pick", "up", "the"} | ({"ball"} if level == BABYAI_MAZE_KEYCORRIDOR else _TYPES))
     if variant == BABYAI_GOTO:  # GoToInstr(ObjDesc(type, colour))
         return frozenset({"go", "to"} | art | _COLORS | _TYPES)
     if variant == BABYAI_PICKUP_PUTNEXT:
@@ -376,9 +411,11 @@ def get(env_id: str) -> EnvSpec:
         return BABYAI_PICKUP_PUTNEXT_REGISTRY[env_id]
     if env_id in BABYAI_OPEN_REGISTRY:
         return BABYAI_OPEN_REGISTRY[env_id]
+    if env_id in BABYAI_MAZE_REGISTRY:
+        return BABYAI_MAZE_REGISTRY[env_id]
     try:
         return REGISTRY[env_id]
     except KeyError:
         raise KeyError(f"{env_id!r} is not one of the ids this engine implements: "
-                       f"{sorted(REGISTRY) + sorted(BABYAI_REGISTRY) + sorted(BABYAI_PICKUP_PUTNEXT_REGISTRY) + sorted(BABYAI_OPEN_REGISTRY)}"
+                       f"{sorted(REGISTRY) + sorted(BABYAI_REGISTRY) + sorted(BABYAI_PICKUP_PUTNEXT_REGISTRY) + sorted(BABYAI_OPEN_REGISTRY) + sorted(BABYAI_MAZE_REGISTRY)}"
                        ) from None
