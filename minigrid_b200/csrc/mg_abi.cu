@@ -18,7 +18,7 @@
 namespace mg {
 cudaError_t launch_step(const Params &p, const StepPlan &plan, const void *actions, int action_dtype, uint8_t *obs,
                         int32_t *dir, double *reward, uint8_t *term, uint8_t *trunc, uint32_t *packed, int step_parity,
-                        cudaStream_t stream);
+                        bool border_walls, cudaStream_t stream);
 cudaError_t configure_step(const Params &p, StepPlan *plan);
 cudaError_t launch_reset(const Params &p, const uint8_t *mask, uint8_t *obs, int32_t *dir, cudaStream_t stream);
 cudaError_t launch_seed(const Params &p, const uint8_t *mask, const uint64_t *seeds_dev, uint64_t base, cudaStream_t stream);
@@ -88,6 +88,9 @@ struct mg_env {
   // mg_enable_missions: allowed while no seed, reset or step has touched the envs; the roomgrid kind then keeps the
   // codes in p.extra (mission_codes()), the other kinds' missions are constant (code 0)
   int touched, missions;
+  // every grid's border cells are walls: true from mg_create (k_init fills the arena with walls) and after a full reset,
+  // false once a grid has been injected. With a walled kind (kind_walled) K1 then skips the border lines.
+  bool border_walls;
 };
 
 static thread_local std::string g_err;
@@ -261,6 +264,7 @@ int mg_create(int kind, int width, int height, int max_steps, int see_through_wa
   p.see_through = see_through_walls ? 1 : 0;
   p.mode = autoreset_mode;
   p.kind = kind;
+  h->border_walls = true;  // k_init fills every grid with walls
   h->trace = getenv("MINIGRID_B200_HOST_TRACE") != nullptr;
   { const char *wp = getenv("MINIGRID_B200_WINPREF"); h->p.win_prefetch = !wp || atoi(wp) != 0; }
   h->stream_fixed = -1;
@@ -485,6 +489,7 @@ int mg_reset(mg_env *h, uint8_t *obs_dev, int32_t *dir_dev, void *stream) {
   h->touched = 1;
   MG_CUDA(launch_reset(h->p, nullptr, obs_dev, dir_dev, s));
   h->launches += 1;
+  h->border_walls = true;
   return MG_OK;
 }
 
@@ -516,7 +521,7 @@ int mg_step(mg_env *h, const void *actions_dev, int action_dtype, uint8_t *obs_d
   }
   // one launch: transition + autoreset (either mode) + observation
   MG_CUDA(launch_step(p, h->plan, actions_dev, action_dtype, obs_dev, dir_dev, reward_dev, terminated_dev,
-                      truncated_dev, nullptr, (int)(h->launches & 1), s));
+                      truncated_dev, nullptr, (int)(h->launches & 1), h->border_walls, s));
   h->launches += 1;
   if (h->profiling) {
     MG_CUDA(cudaEventRecord(ev1, s));
@@ -531,7 +536,7 @@ int mg_gen_obs(mg_env *h, uint8_t *obs_dev, int32_t *dir_dev, void *stream) {
   MG_ON_DEVICE(h);
   note_stream(h, (cudaStream_t)stream);
   MG_CUDA(launch_step(h->p, h->plan, nullptr, MG_ACT_I32, obs_dev, dir_dev, nullptr, nullptr, nullptr, nullptr, 0,
-                      (cudaStream_t)stream));
+                      h->border_walls, (cudaStream_t)stream));
   h->launches += 1;
   return MG_OK;
 }
@@ -718,6 +723,7 @@ int mg_set_state(mg_env *h, const uint8_t *grid_dev, const int32_t *agent_dev, c
   note_stream(h, s);
   MG_CUDA(launch_set_state(h->p, grid_dev, agent_dev, rng_dev, pending_dev, s));
   h->launches += (grid_dev ? 1 : 0) + ((agent_dev || rng_dev || pending_dev) ? 1 : 0);
+  if (grid_dev) h->border_walls = false;  // an injected grid may have anything on its border, until the next full reset
   if (agent_dev) {
     // K1 trusts the agent records (window offsets, bit-mask shifts): records that fail the range checks were not
     // stored (k_set_agent) and are reported here; this makes an agent injection synchronous.
@@ -883,7 +889,7 @@ static int step_host_packed(mg_env *h, const int32_t *src, uint8_t *obs_host, in
   pool->begin(job, bounds, C);  // the workers wake up while the copy and the kernel run
   cudaError_t e = cudaMemcpyAsync(h->d_actions, src, n * sizeof(int32_t), cudaMemcpyHostToDevice, s);
   if (e == cudaSuccess)
-    e = launch_step(h->p, h->plan, h->d_actions, MG_ACT_I32, nullptr, nullptr, nullptr, nullptr, nullptr, h->d_packed, (int)(h->launches & 1), s);
+    e = launch_step(h->p, h->plan, h->d_actions, MG_ACT_I32, nullptr, nullptr, nullptr, nullptr, nullptr, h->d_packed, (int)(h->launches & 1), h->border_walls, s);
   h->launches += 1;
   for (int c = 0; c < C && e == cudaSuccess; ++c) {
     const size_t off = (size_t)bounds[c] * PACKED_BYTES, len = (size_t)(bounds[c + 1] - bounds[c]) * PACKED_BYTES;

@@ -77,6 +77,13 @@ enum : int { KIND_EMPTY = 0, KIND_DOORKEY = 1, KIND_CROSSING = 2, KIND_FOURROOMS
              // SURVEY 8(f-2), second half: core/roomgrid.py with unlock.py, unlockpickup.py, blockedunlockpickup.py, keycorridor.py
              KIND_ROOMGRID = 16 };
 constexpr int KIND_COUNT = 17;
+// Kinds whose grids keep grey walls on the whole border: the generator starts with wall_rect(0, 0, W, H) and places
+// nothing on the border, there is no step post-filter and no draw inside step (Dynamic-Obstacles re-places its
+// obstacles anywhere), and no action changes a wall. K1 then does not stage the border lines of their tiles
+// (mg_step_kernel.cuh: stage_lines) while no grid has been injected (mg_set_state).
+MG_HD constexpr bool kind_walled(int kind) {
+  return kind == KIND_EMPTY || kind == KIND_DOORKEY || kind == KIND_CROSSING || kind == KIND_LAVAGAP || kind == KIND_DISTSHIFT;
+}
 // kp[0] of KIND_ROOMGRID; the ObstructedMaze variants (envs/obstructedmaze.py, obstructedmaze_v1.py) also read
 // kp[4] key_in_box, kp[5] blocked, kp[6] agent room i | j << 4, kp[7] num_quarters
 enum : int { RG_UNLOCK = 0, RG_UNLOCKPICKUP = 1, RG_BLOCKEDUNLOCKPICKUP = 2, RG_KEYCORRIDOR = 3, RG_OBSTRUCTED_1D = 4,

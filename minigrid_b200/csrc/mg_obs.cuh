@@ -7,7 +7,7 @@
 //                                                          line of array R (dir 0/2) or C (dir 1/3), read
 //                                                          forwards or backwards: 3 word loads + 2 funnel
 //                                                          shifts + 2 byte permutes per column
-//   out of bounds -> Wall()      (grid.py:136-139)         ring lines + a per-step byte mask
+//   out of bounds -> Wall()      (grid.py:136-139)         per-column line mask + a per-step byte mask
 //   Grid.process_vis             (grid.py:291-328)         49-bit boards (byte = view row, bit = view column):
 //                                                          carry-chain fill rightwards, Kogge-Stone leftwards
 //   carry overlay                (minigrid_env.py:623-630) one byte permute
@@ -19,9 +19,13 @@
 namespace mg {
 
 // Word accessors: gen_obs_words asks for word w of the environment (w as in r_word / c_word).
+// `edge`: only lines [edge, n - 1 - edge] of each array may be read (n = H lines of R, W lines of C). 0: every grid line,
+// the ring lines never; 1 (K1 on a walled level, mg_step_kernel.cuh: stage_lines): not the border lines either. The
+// gather reads every line outside that range as a grey wall, which is what those lines hold.
 struct AccTiled {   // LAYOUT_TILED, lane column of a tile in shared (K1) or global (K2) memory: word w at base[w * 32]
   const uint32_t *base;
   bool smem;
+  int edge = 0;
   MG_D uint32_t operator()(int w) const {
 #ifdef __CUDA_ARCH__
     if (smem) {
@@ -35,6 +39,7 @@ struct AccTiled {   // LAYOUT_TILED, lane column of a tile in shared (K1) or glo
 };
 struct AccFlat {    // LAYOUT_WINDOW: env-major words; `base` is shifted so that base[w] is word w (global memory in
   const uint32_t *base;  // K2; in K1 the lane's 7-line window in shared memory, shifted by its first word index)
+  int edge = 0;
   MG_D uint32_t operator()(int w) const { return base[w]; }
 };
 // kept for the transition's single front-cell read out of a staged tile
@@ -42,6 +47,17 @@ template <bool SMEM>
 MG_D uint32_t tile_word(const uint32_t *base, int w) {
   AccTiled a = {base, SMEM};
   return a(w);
+}
+// The cell at position `pos` of the agent's own line: line ay of array R when it faces +-x (dir 0 / 2), line ax of array
+// C when it faces +-y. That line is readable for every agent that stands inside the readable lines; a line outside them
+// (an agent record injected onto the border of a walled level) or a position outside the grid reads as a grey wall.
+template <class Acc>
+MG_D uint32_t own_line_cell(const Geom &g, const Acc &acc, int ax, int ay, int dir, int pos) {
+  const bool useC = dir & 1;
+  const int l = useC ? ax : ay, nlines = useC ? g.W : g.H, plen = useC ? g.H : g.W;
+  if ((unsigned)(l - acc.edge) >= (unsigned)(nlines - 2 * acc.edge) || (unsigned)pos >= (unsigned)plen) return CODE_WALL;
+  const int w = (useC ? g.offC : 0) + (l + g.ring) * (useC ? g.lswC : g.lswR) + (pos >> 2);
+  return (acc(w) >> (8 * (pos & 3))) & 0xFFu;
 }
 
 // One row of Grid.process_vis (grid.py:291-328) on 7-bit masks (bit i = view column i): m = cells of this row
@@ -139,8 +155,10 @@ MG_D void gather_view(const Geom &g, const Acc &acc, const uint16_t *vis_tbl, in
   uint32_t oplo = 0, ophi = 0;
 #pragma unroll
   for (int vx = 0; vx < VIEW; ++vx) {
-    const int l = clampi(lc + lstep * (vx - 3), -g.ring, nlines + g.ring - 1) + g.ring;
-    const int rw = abase + l * lsw;
+    // a view column on a line the accessor may not read is a wall line: past the grid (Grid.slice) or a walled border
+    const int lv = lc + lstep * (vx - 3);
+    const int l = clampi(lv, acc.edge, nlines - 1 - acc.edge);
+    const int rw = abase + (l + g.ring) * lsw;
     const uint32_t w0 = acc(rw + k0);
     const uint32_t w1 = acc(rw + k1);
     const uint32_t w2 = acc(rw + k2);
@@ -148,8 +166,9 @@ MG_D void gather_view(const Geom &g, const Acc &acc, const uint16_t *vis_tbl, in
     const uint32_t b = __funnelshift_r(w1, w2, sh);
     uint32_t lo = prmt(a, b, selLo);
     uint32_t hi = prmt(a, b, selHi);
-    lo = (lo & mlo) | (CODE_WALL4 & ~mlo);
-    hi = (hi & mhi) | ((CODE_WALL4 & 0x00FFFFFFu) & ~mhi);
+    const uint32_t ml = l == lv ? mlo : 0u, mh = l == lv ? mhi : 0u;
+    lo = (lo & ml) | (CODE_WALL4 & ~ml);
+    hi = (hi & mh) | ((CODE_WALL4 & 0x00FFFFFFu) & ~mh);
     clo[vx] = lo; chi[vx] = hi;
     if (VIS != VIS_NONE) {
       oplo |= ((lo >> 7) & 0x01010101u) << vx;

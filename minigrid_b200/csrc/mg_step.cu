@@ -2,8 +2,9 @@
 // vector-level autoreset (MiniGridEnv.reset, :119-157) for a batch: ONE launch per vector step.
 //
 // One warp = one tile of 32 environments, one lane per environment.
-//   1. lane 0 issues a TMA bulk copy (cp.async.bulk -> SASS UBLKCP) of the tile's interleaved grid words
-//      into shared memory and arms an mbarrier with the byte count; meanwhile every lane loads its
+//   1. lane 0 issues TMA bulk copies (cp.async.bulk -> SASS UBLKCP) of the tile's interleaved grid lines that the step
+//      can read (stage_lines: no ring lines; no border lines on a walled level) into shared memory and arms an mbarrier
+//      with the byte count; meanwhile every lane loads its
 //      action and 16-byte agent record with coalesced loads. Warps are persistent (one CTA per SM, one wave). Default
 //      plan: one buffer per warp, 22 warps at 72 registers (mg_step_tiled1.cu); the two-buffer form, in which a warp
 //      requests its next tile (copy + records + actions) while it works on the current one, is this file's (configure_step).
@@ -108,9 +109,10 @@ cudaError_t configure_step(const Params &p, StepPlan *plan) {
 
 cudaError_t launch_step(const Params &p, const StepPlan &plan, const void *actions, int action_dtype, uint8_t *obs,
                         int32_t *dir, double *reward, uint8_t *term, uint8_t *trunc, uint32_t *packed, int step_parity,
-                        cudaStream_t stream) {
+                        bool border_walls, cudaStream_t stream) {
   int tma_ok = ((reinterpret_cast<uintptr_t>(obs) & 15u) == 0) ? 1 : 0;
   tma_ok |= (step_parity & 1) << 2;  // direction of the unflagged tiles in K1's order list
+  if (border_walls && kind_walled(p.kind)) tma_ok |= 8;  // K1 stages the tiles without their border lines
 #ifdef MG_TIMELINE
   static int launch_no = 0;
   tma_ok |= (launch_no++ & 1) << 1;

@@ -76,6 +76,16 @@ __device__ __forceinline__ void tma_load_1d(uint32_t dst, const void *src, uint3
                "l"(src), "r"(bytes), "r"(bar)
                : "memory");
 }
+// Stage the grid lines of a tile that the step can read into a tiled buffer, at their usual offsets (r_word / c_word
+// index the buffer as before): lines [edge, n - 1 - edge] of array R, then the same line range of array C. The ring
+// lines are never read (gather_view reads past the grid as wall), nor are the border lines of a walled handle (edge 1).
+__device__ __forceinline__ void stage_lines(const Geom &g, int edge, uint32_t dst, const uint32_t *tile_src, uint32_t bar) {
+  const uint32_t r0 = (uint32_t)r_word(g, 0, edge), nr = (uint32_t)((g.H - 2 * edge) * g.lswR);
+  const uint32_t c0 = (uint32_t)c_word(g, edge, 0), nc = (uint32_t)((g.W - 2 * edge) * g.lswC);
+  mbar_expect_tx(bar, (nr + nc) * 128u);
+  tma_load_1d(dst + r0 * 128u, tile_src + r0 * 32u, nr * 128u, bar);
+  tma_load_1d(dst + c0 * 128u, tile_src + c0 * 32u, nc * 128u, bar);
+}
 __device__ __forceinline__ void tma_store_1d(void *dst, uint32_t src, uint32_t bytes) {
   asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(src), "r"(bytes) : "memory");
 }
@@ -284,7 +294,8 @@ k_step(const __grid_constant__ Params p, const void *__restrict__ actions, int a
   g.ring = WIN ? 3 : 1;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int WARPS = blockDim.x >> 5;
-  const uint32_t tile_bytes = (uint32_t)g.wpe * 128u;
+  // bit 3 of obs_tma_ok: no grid of the handle has been injected, so a walled kind's border lines are walls
+  const int edge = (kind_walled(KIND) && (obs_tma_ok & 8)) ? 1 : 0;
   const uint32_t buf_bytes = step_buf_bytes(g);
   constexpr uint32_t TBL = (VIS == VIS_TBL) ? (uint32_t)VIS_TBL_BYTES : 0u;
 
@@ -383,10 +394,7 @@ k_step(const __grid_constant__ Params p, const void *__restrict__ actions, int a
   uint4 rec = make_uint4(0, 0, 0, 0);
   int action = A_DONE;
   if (PREF && tile < p.n_tiles) {
-    if (NBUF == 2 && lane == 0) {
-      mbar_expect_tx(bar0, tile_bytes);
-      tma_load_1d(smem_u32(bufs), p.grid + (size_t)tile * g.wpe * 32, tile_bytes, bar0);
-    }
+    if (NBUF == 2 && lane == 0) stage_lines(g, edge, smem_u32(bufs), p.grid + (size_t)tile * g.wpe * 32, bar0);
     const int env0 = tile * TILE + lane;
     rec = ldg_rec(p.agent + env0);
     if (stepping && env0 < p.n_envs) action = load_action(actions, act_dtype, env0);
@@ -406,9 +414,7 @@ k_step(const __grid_constant__ Params p, const void *__restrict__ actions, int a
         if (lane == 0) {
           if (NBUF == 2) {
             asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // the obs block staged there two tiles ago
-            const uint32_t nb = bar0 + 8u * (uint32_t)(b ^ 1);
-            mbar_expect_tx(nb, tile_bytes);
-            tma_load_1d(smem_u32(bufs + (size_t)(b ^ 1) * buf_bytes), p.grid + (size_t)next * g.wpe * 32, tile_bytes, nb);
+            stage_lines(g, edge, smem_u32(bufs + (size_t)(b ^ 1) * buf_bytes), p.grid + (size_t)next * g.wpe * 32, bar0 + 8u * (uint32_t)(b ^ 1));
           }
           nn = map_tile(atomicAdd(s_next, 1));  // shared-memory atomic, consumed one tile later
         }
@@ -427,8 +433,7 @@ k_step(const __grid_constant__ Params p, const void *__restrict__ actions, int a
     } else {
       if (lane == 0) {
         asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // the previous obs block has left the buffer
-        mbar_expect_tx(bar0, tile_bytes);
-        tma_load_1d(smem_u32(bufs), p.grid + (size_t)tile * g.wpe * 32, tile_bytes, bar0);
+        stage_lines(g, edge, smem_u32(bufs), p.grid + (size_t)tile * g.wpe * 32, bar0);
       }
       const int env0 = tile * TILE + lane;
       rec = ldg_rec(p.agent + env0);
@@ -465,6 +470,7 @@ k_step(const __grid_constant__ Params p, const void *__restrict__ actions, int a
     }
 
     const uint32_t *base = gtile + lane;
+    const AccTiled tacc = {base, true, edge};  // the staged lines of this lane's env
     double reward = 0.0;
     uint32_t terminated = 0, truncated = 0;
     int rsteps = 0;  // the step count the reward was computed from (a SAME_STEP autoreset zeroes `steps` afterwards)
@@ -539,7 +545,7 @@ k_step(const __grid_constant__ Params p, const void *__restrict__ actions, int a
       uint32_t fc;
       const int fpos = ((dir & 1) ? ay : ax) + ((dir < 2) ? 1 : -1);  // the front cell's position on the agent's own line
       if (WIN) fc = view_words_byte(vw, fpos);  // meaningless after a turn (other array loaded), and then unused
-      else fc = (tile_word<true>(base, rw) >> (8 * (fx & 3))) & 0xFFu;
+      else fc = own_line_cell(g, tacc, ax, ay, dir, (dir & 1) ? fy : fx);
 
       const uint32_t carry_before = carry;
       const int act = pre_filter<KIND>(action);
@@ -585,8 +591,7 @@ k_step(const __grid_constant__ Params p, const void *__restrict__ actions, int a
           if (WIN) {  // the loaded words hold the agent's line for its new direction, the mutation included
             in.front = view_words_byte(vw, ((dir & 1) ? ay : ax) + ((dir < 2) ? 1 : -1));
           } else {
-            const int nx = ax + (dir == 0) - (dir == 2), ny = ay + (dir == 1) - (dir == 3);
-            in.front = (tile_word<true>(base, r_word(g, nx, ny)) >> (8 * (nx & 3))) & 0xFFu;
+            in.front = own_line_cell(g, tacc, ax, ay, dir, ((dir & 1) ? ay : ax) + ((dir < 2) ? 1 : -1));
           }
         }
         in.level = p.kp[4]; in.next_to = 0;
@@ -625,7 +630,7 @@ k_step(const __grid_constant__ Params p, const void *__restrict__ actions, int a
         uint32_t cur = 0;  // the cell under the agent after the step
         if (p.no_death_mask) {
           if (WIN) cur = view_words_byte(vw, (dir & 1) ? ay : ax);
-          else cur = (tile_word<true>(base, r_word(g, ax, ay)) >> (8 * (ax & 3))) & 0xFFu;
+          else cur = own_line_cell(g, tacc, ax, ay, dir, (dir & 1) ? ay : ax);
         }
         const WrapOut wo = wrap_step(p, env, active, action_raw, (KIND == KIND_DYNOBS && !WIN) ? fc_before : fc, cur, ax, ay, dir, reward, terminated);
         reward = wo.reward;
@@ -674,8 +679,7 @@ k_step(const __grid_constant__ Params p, const void *__restrict__ actions, int a
       if (WIN) {
         gather_from_words<VIS>(g, vw, vis_tbl, ax, ay, dir, carry, clo, chi);
       } else {
-        const AccTiled acc = {base, true};
-        gather_view<VIS>(g, acc, vis_tbl, ax, ay, dir, carry, clo, chi);
+        gather_view<VIS>(g, tacc, vis_tbl, ax, ay, dir, carry, clo, chi);
       }
       const int nvalid = min(TILE, p.n_envs - tile * TILE);
       if (packed_out == nullptr) {
